@@ -1,10 +1,11 @@
 #!/usr/bin/env python
-"""Headline benchmark: pipelined ViT / BERT / DeiT inference throughput on N B200s (one stage per GPU).
+"""Headline benchmark: pipelined ViT / BERT / DeiT inference throughput on N H100s (one stage per GPU).
 
     python bench.py --gpus 1 --steps 200 --warmup 20                       # N = 1
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W                             # N > 1, one rank per GPU
     python bench.py --impl reference --gpus N --steps K --warmup W         # the reference's CPU path
+    python bench.py --gpus 1 --steps K --warmup W --dump-outputs DIR       # + the last timed step's logits as .npy
 
 A STEP is one micro-batch through the whole pipeline (BASELINE.json: images/s or sequences/s per pipeline).
 Default workload = BASELINE.json configs[1]'s model and micro-batch (google/vit-base-patch16-224, ubatch 8,
@@ -21,12 +22,16 @@ One JSON line is printed by rank 0:
   e2e          the same through the public API with pinned HOST inputs: H2D of every micro-batch and D2H of
                every result inside the (wall-clock, device-synchronised) timed region
   checksum     sum |logits| over the first 16 results: identical inputs at every N, so it must not depend on N
-  roofline     N = 1: the dominant kernel (the FC1 tcgen05 GEMM): algorithmic FLOPs per launch / its CUDA-event
-               duration, against MEASURED_PEAKS.json; N > 1: the bottleneck STAGE (its GEMM + attention FLOPs over its
+  roofline     N = 1: the dominant kernel (the FC1 wgmma GEMM): algorithmic FLOPs per launch / its CUDA-event
+               duration, against MEASURED_PEAKS.json or the H100 SXM data sheet; N > 1: the bottleneck STAGE (its GEMM + attention FLOPs over its
                event-timed kernel sequence), per-rank breakdown under `stages`
-  cpu_baseline the CPU oracle port (oracle/shards.py, torch fp32 on the host cores) on a bounded sample
+  cpu_baseline the CPU oracle port (oracle/shards.py, torch fp32 on the host cores) on 24 micro-batches
 `--impl reference` times that CPU port as the reference arm with the same thread calibration and the same `config`
-(the reference is Python and cannot travel to the GPU box; see DESIGN.md).
+(the reference is Python and cannot travel to the GPU machine; see DESIGN.md).
+`--dump-outputs DIR` writes, after the timed steps, the logits of the last timed micro-batch as DIR/logits.npy
+(float32): what the data rank received (GPU arm), what the last shard call returned (`--quick`) or what the CPU port
+computed (`--impl reference`). Inputs and weights come from fixed seeds, so two builds run with the same arguments can
+be compared output for output.
 """
 import argparse
 import faulthandler
@@ -156,8 +161,8 @@ def load_peaks() -> dict:
             peaks = json.load(fh)
         peaks['source'] = 'measured'
         return peaks
-    # /opt/skills/guides/B200_PROFILING.md fallback
-    return {'hbm_gbs': 6650.0, 'bf16_tflops': 1590.0, 'bf16_tflops_sustained': 1400.0, 'source': 'fallback'}
+    # NVIDIA's H100 SXM data sheet (dense BF16 at up to 700 W): a ceiling, not a rate this card was measured to reach
+    return {'hbm_gbs': 3350.0, 'bf16_tflops': 989.0, 'bf16_tflops_sustained': 989.0, 'source': 'H100 SXM data sheet'}
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -212,12 +217,12 @@ def cpu_forward_timer(spec, ubatch: int, seq: int):
                                               'median_s_by_threads': {str(k): round(v, 4) for k, v in log.items()}}
 
 
-def cpu_sample(spec, ubatch: int, seq: int, unit: str, max_steps: int, budget_s: float) -> dict:
-    """Time the CPU port on a bounded sample; the same routine serves `cpu_baseline` and `--impl reference`."""
+def cpu_sample(spec, ubatch: int, seq: int, unit: str, steps: int) -> dict:
+    """Time `steps` forwards of the CPU port; the same routine serves `cpu_baseline` and `--impl reference`."""
     fwd, cores, cal = cpu_forward_timer(spec, ubatch, seq)
     # Warm-up until the per-forward time has settled: the first forwards of a process run ~2x slower than its steady state
-    # (the allocator still maps and unmaps the 10-100 MB temporaries of every layer; r02g: 0.31 s vs 0.14 s per
-    # micro-batch), which is why a 20-step arm and a 64-step arm of the same code disagreed by 2x.
+    # (the allocator still maps and unmaps the 10-100 MB temporaries of every layer), so a short arm and a long arm of
+    # the same code would disagree.
     t_w = time.perf_counter()
     warm, last = 0, float('inf')
     while warm < 40 and time.perf_counter() - t_w < 12.0:
@@ -230,13 +235,12 @@ def cpu_sample(spec, ubatch: int, seq: int, unit: str, max_steps: int, budget_s:
         last = min(last, dt1)
     cal['warmup_forwards'] = warm
     t0 = time.perf_counter()
-    n = 0
-    while n < 2 or (n < max_steps and time.perf_counter() - t0 < budget_s):
-        fwd()
-        n += 1
+    for _ in range(steps):
+        logits = fwd()
     dt = time.perf_counter() - t0
+    n = steps
     return {'value': n * ubatch / dt, 'unit': unit, 'cores': cores, 'kind': 'port', 'steps': n, 'seconds': dt,
-            'calibration': cal,
+            'calibration': cal, 'logits': logits,
             'sample': f"{n} micro-batches of {ubatch} through all {spec.layers} sub-layers, torch fp32 CPU "
                       f"({dt:.1f} s), 1 process x {cores} threads of {cal['host_cores']} usable host cores "
                       "(median-of-3 thread calibration)"}
@@ -245,12 +249,9 @@ def cpu_sample(spec, ubatch: int, seq: int, unit: str, max_steps: int, budget_s:
 def cpu_baseline_child(args) -> dict:
     """`cpu_baseline` of the GPU arm = the reference arm's own command in a child process.
 
-    The CPU port's speed depends on the state of the process it runs in: on the B200 hosts (2 x Xeon 8562Y+, 16-CPU
-    quota) a fresh process needs 0.30 s per ViT-B micro-batch, forward after forward, while the same code at the end of
-    the GPU arm's process needed 0.14 s (scripts/cpu_arm_trajectory.py, profiles/r02_cpu_arm_trajectory.txt; neither a
-    CUDA context created first nor NUMA pinning reproduces the fast regime reliably). Round 1's two CPU numbers differed by
-    2-3x for that reason. Both arms now run the SAME command in the SAME kind of process, so they agree; the faster regime
-    is documented in DESIGN.md section 7 and would halve every GPU / CPU ratio."""
+    The CPU port's speed depends on the state of the process it runs in (a fresh process can be ~2x slower per
+    micro-batch than one that has already run many forwards; scripts/cpu_arm_trajectory.py shows the trajectory), so both
+    arms run the SAME command in the SAME kind of process and agree."""
     cmd = [sys.executable, os.path.abspath(__file__), '--impl', 'reference', '--workload', args.workload, '--steps', '24',
            '--warmup', '2', '--gpus', '1']
     if args.ubatch:
@@ -277,7 +278,9 @@ def run_reference_arm(args, spec, ubatch, seq, qbit, metric, unit, workload):
     if rank != 0:
         return   # the CPU arm is a single process using the host cores; other ranks have no work
     world = int(os.environ.get('WORLD_SIZE', str(args.gpus)))
-    res = cpu_sample(spec, ubatch, seq, unit, max_steps=max(2, args.steps), budget_s=120.0)
+    res = cpu_sample(spec, ubatch, seq, unit, args.steps)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {'logits': res['logits']})
     print(json.dumps({
         'impl': 'reference', 'metric': metric, 'value': res['value'], 'unit': unit, 'n_gpus': args.gpus,
         'steps': res['steps'], 'warmup': args.warmup, 'ms_per_step': res['seconds'] / res['steps'] * 1e3,
@@ -307,7 +310,7 @@ def make_shard(spec, weights, layer_start, layer_end):
 def dominant_kernel_us(spec, ubatch, seq, dev) -> float:
     """Average launch duration (us) of the dominant kernel - the FC1 GEMM with its GELU epilogue - as it runs inside a
     step: back-to-back launches in a CUDA graph (as in the stage's graph), each on a different weight copy so that the
-    weights stream from HBM like in a forward (copies total > 126 MB L2), CUDA events on the launching stream."""
+    weights stream from HBM like in a forward (copies total > 50 MB L2), CUDA events on the launching stream."""
     from pipeedge_b200 import _lib, ops
     m, n, k = ubatch * seq, spec.inter, spec.hidden
     copies = max(8, int(200e6 // (n * k * 2)) + 1)
@@ -364,15 +367,9 @@ def roofline_from_profile(shard, sample, spec, ubatch, seq, peaks, step_ms=None)
     achieved = flops[dom] / (dom_us * 1e-6) / 1e12
     peak = peaks['bf16_tflops_sustained']   # timed inside a long step
     launches = breakdown[dom]['launches_per_forward']
-    traffic = None   # DRAM bytes per launch of this kernel from the committed `ncu --set full` capture
-    try:
-        with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'profiles', 'ncu_traffic.json')) as f:
-            traffic = json.load(f)['dram_bytes_per_launch']
-    except (OSError, KeyError, ValueError):
-        pass
-    return {'bound': 'tensor', 'kernel': 'gemm_tcgen05_kernel<PE_EPI_GELU_F16> (FC1)', 'achieved': achieved,
-            'peak': peak, 'unit': 'TFLOP/s', 'frac': achieved / peak, 'traffic': traffic,
-            'peak_source': f"{peaks['source']} bf16_tflops_sustained (MEASURED_PEAKS.json)",
+    return {'bound': 'tensor', 'kernel': 'gemm_wgmma_kernel<PE_EPI_GELU_F16> (FC1)', 'achieved': achieved,
+            'peak': peak, 'unit': 'TFLOP/s', 'frac': achieved / peak, 'traffic': None,
+            'peak_source': f"{peaks['source']} bf16_tflops_sustained",
             'flops_per_launch': flops[dom], 'avg_launch_us': dom_us,
             'method': 'CUDA events around a graph of back-to-back launches on distinct weight copies (> L2)',
             'share_of_step': (launches * dom_us * 1e-3 / step_ms) if step_ms else sum(acc[dom]) / 3 / total_ms,
@@ -488,7 +485,7 @@ def run_gpu(args, spec, ubatch, seq, qbit, metric, unit, workload):
             native = stage_ctx.native
             if native is None:
                 raise SystemExit("bench.py: the native pipeline was not selected (PIPEEDGE_NATIVE=0 or a rank without a "
-                                 "B200 shard?)")
+                                 "native shard?)")
             stage_ctx.prepare(ubatch, dim1)          # graph capture happens here, before any timed or warm-up step
             inputs_host = inputs_dev = None
             if rank == 0:
@@ -543,6 +540,8 @@ def run_gpu(args, spec, ubatch, seq, qbit, metric, unit, workload):
             run_phase(max(extra, 1), False)
             _, tim = run_phase(steps, False)
             clocks.mark_end()
+            if rank == 0 and args.dump_outputs:   # the last timed micro-batch's logits, before later phases refill `got`
+                dump_outputs(args.dump_outputs, {'logits': got[-1]})
             clocks.__exit__(None, None, None)
             ms_rank = max(tim['compute_ms'], tim['results_ms'])
             ms = allmax(ms_rank)
@@ -581,7 +580,7 @@ def run_gpu(args, spec, ubatch, seq, qbit, metric, unit, workload):
                                  'l2': f"timed loop rotates over {N_INPUTS} distinct resident micro-batches"
                                        + ("; the stage's fp16 weights "
                                           f"({spec.blocks * (4 * spec.hidden ** 2 + 2 * spec.hidden * spec.inter) * 2 / 1e6:.0f} MB) "
-                                          "exceed the 126 MB L2 and stream from HBM every step" if world == 1 else
+                                          "exceed the 50 MB L2 and stream from HBM every step" if world == 1 else
                                           "; per-stage weights may be L2-resident, as in steady-state serving")},
                     'clocks': clocks.summary(),
                     'e2e': {'value': steps * ubatch / e2e_wall, 'unit': unit, 'h2d_bytes_per_step': h2d,
@@ -599,7 +598,7 @@ def run_gpu(args, spec, ubatch, seq, qbit, metric, unit, workload):
                         out['roofline'] = roofline_from_profile(shard, emb, spec, ubatch, seq_eff, peaks, step_ms=ms / steps)
                 else:
                     worst = max(stages, key=lambda st: st['eager_ms'])
-                    out['roofline'] = {'bound': 'tensor', 'kernel': f"bottleneck stage {worst['layers']} (tcgen05 GEMMs + attention)",
+                    out['roofline'] = {'bound': 'tensor', 'kernel': f"bottleneck stage {worst['layers']} (wgmma GEMMs + attention)",
                                        'achieved': worst['tflops'], 'peak': peaks['bf16_tflops_sustained'], 'unit': 'TFLOP/s',
                                        'frac': worst['tflops'] / peaks['bf16_tflops_sustained'], 'traffic': None,
                                        'note': 'stage FLOPs / sum of its event-bracketed kernel times (upper bound on time); the '
@@ -613,6 +612,16 @@ def run_gpu(args, spec, ubatch, seq, qbit, metric, unit, workload):
         if not args.no_cpu_baseline and world == 1:
             out['cpu_baseline'] = cpu_baseline_child(args)
         print(json.dumps(out))
+
+
+def dump_outputs(out_dir: str, arrays: dict) -> None:
+    """Write each tensor as out_dir/<name>.npy in float32 (float64 stays float64)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        a = t.detach().cpu()
+        a = a.double() if a.dtype == torch.float64 else a.float()
+        np.save(os.path.join(out_dir, f'{name}.npy'), a.numpy())
 
 
 def run_quick(args, spec, ubatch, seq):
@@ -632,9 +641,11 @@ def run_quick(args, spec, ubatch, seq):
         start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         start.record(stream)
         for i in range(args.steps):
-            shard(xs[i % 4])
+            out = shard(xs[i % 4])
         end.record(stream)
         torch.cuda.synchronize()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {'logits': out})
     ms = start.elapsed_time(end)
     print(json.dumps({'quick': True, 'value': args.steps * ubatch / (ms * 1e-3), 'ms_per_step': ms / args.steps,
                       'gpu_launches': int(ops.launch_count() - l0)}))
@@ -644,7 +655,8 @@ def main():
     faulthandler.enable()   # a native crash in any thread prints every thread's Python stack to stderr
     ap = argparse.ArgumentParser()
     ap.add_argument('--gpus', type=int, default=1)
-    ap.add_argument('--steps', type=int, default=300)
+    ap.add_argument('--steps', type=int, default=None,
+                    help='timed steps (micro-batches); default 300 on the GPU, 24 for the CPU arm (--impl reference)')
     ap.add_argument('--warmup', type=int, default=20)
     ap.add_argument('--impl', choices=['ours', 'reference'], default='ours')
     ap.add_argument('--workload', choices=sorted(WORKLOADS), default='vit-base')
@@ -652,13 +664,17 @@ def main():
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--quick', action='store_true', help='only a resident-input loop of direct shard calls (for ncu runs)')
     ap.add_argument('--eager', action='store_true', help='with --quick: no CUDA graph (every kernel visible to ncu)')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write the last timed micro-batch\'s logits to DIR/logits.npy')
     args = ap.parse_args()
     model, ubatch, seq, qbit, metric, unit = WORKLOADS[args.workload]
     ubatch = args.ubatch or ubatch
     spec = MODEL_SPECS[model]
+    if args.steps is None:
+        args.steps = 24 if args.impl == 'reference' else 300
+    if args.steps < 1:
+        ap.error('--steps must be at least 1')
     if args.impl == 'reference':
-        if args.steps == 300:
-            args.steps = 24   # a bounded CPU sample by default
         run_reference_arm(args, spec, ubatch, seq, qbit, metric, unit, args.workload)
         return
     if not torch.cuda.is_available():

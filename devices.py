@@ -1,6 +1,6 @@
 """Common device configuration - same module surface as the reference `devices.py`.
 
-On the B200 path activations never leave the GPU between the shard and the hop, so the two hooks the
+On the native GPU path activations never leave the GPU between the shard and the hop, so the two hooks the
 reference installs around every shard forward (`devices.py:8-24`: H2D before, D2H after) are identities:
 host inputs of the data rank are staged by the shard itself on a copy stream (see
 `pipeedge_b200/models/transformers/_shard.py`), and there is no CPU fallback to move results to.

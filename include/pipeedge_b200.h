@@ -1,4 +1,4 @@
-/* pipeedge_b200 - C-ABI of the B200-native PipeEdge hot path.
+/* pipeedge_b200 - C-ABI of the H100-native PipeEdge hot path.
  *
  * The reference (usc-isi/PipeEdge @ 1a68bbb) has no C/FFI boundary on this path: it sits behind three
  * PYTHON contracts (SURVEY.md 8b). This header is the boundary we define beneath them; each entry
@@ -13,7 +13,7 @@
  *    "f32" = IEEE binary32, "f16" = IEEE binary16, "u8" = bytes;
  *  - `stream` is a `cudaStream_t` passed as `void*`; calls only enqueue work and never synchronise;
  *  - no global mutable state besides per-handle state; callable with the Python GIL released;
- *  - the library targets sm_100a only and refuses to run elsewhere (PE_ERR_DEVICE).
+ *  - the library targets sm_90a (H100) only and refuses to run elsewhere (PE_ERR_DEVICE).
  */
 #ifndef PIPEEDGE_B200_H
 #define PIPEEDGE_B200_H
@@ -28,7 +28,7 @@ extern "C" {
 #define PE_OK 0
 #define PE_ERR_INVALID (-1) /* bad argument / unsupported shape */
 #define PE_ERR_CUDA (-2)    /* a CUDA runtime or driver call failed */
-#define PE_ERR_DEVICE (-3)  /* no sm_100 device */
+#define PE_ERR_DEVICE (-3)  /* no sm_90 device */
 #define PE_ERR_NOMEM (-4)
 
 #define PE_ABI_VERSION 2
@@ -70,13 +70,13 @@ int pe_layernorm(const void* x, const void* gamma, const void* beta, float eps, 
 int pe_residual_layernorm(const void* y, const void* resid, const void* gamma, const void* beta, float eps,
                           void* sum_out, void* out_f32, void* out_f16, int rows, int hidden, void* stream);
 
-/* ---- Dense contraction `out = epilogue(A @ W^T + bias)` on tcgen05 tensor cores ---------------
+/* ---- Dense contraction `out = epilogue(A @ W^T + bias)` on wgmma tensor cores ---------------
  * Replaces every `nn.Linear` on the path (`ViTSelfAttention.query/key/value`, `ViTSelfOutput.dense`,
  * `ViTIntermediate.dense`, `ViTOutput.dense` and the Bert equivalents; reference call sites
  * `vit.py:60-69`, `bert.py:45-51`).
  * a f16 [m, k]; w f16 [n, k] (the `nn.Linear.weight` layout); bias f32 [n] or NULL;
  * resid f32 [m, n] (PE_EPI_RESID_F32 only; may alias `out`); out [m, n] f16 or f32 per epilogue.
- * Requires k % 8 == 0 (16-byte TMA row pitch). fp32 accumulation in TMEM. */
+ * Requires k % 8 == 0 (16-byte TMA row pitch). fp32 accumulation in registers. */
 int pe_linear(const void* a, const void* w, const void* bias, const void* resid, void* out, int m, int n, int k,
               int epilogue, void* stream);
 
@@ -204,7 +204,7 @@ int pe_stage_kernel_count(const pe_stage* stage);
 
 /* ---- Stage-0 edges (SURVEY.md 8a-A13) ------------------------------------------------------------
  * pe_patch_embed replaces HF `ViTEmbeddings` / `DeiTEmbeddings` as used at `vit.py:96,165`, `deit.py:95,161`:
- * Conv2d(C, H, P, stride P) as an im2col + tcgen05 GEMM whose epilogue adds the conv bias and position
+ * Conv2d(C, H, P, stride P) as an im2col + wgmma GEMM whose epilogue adds the conv bias and position
  * rows and scatters into token rows n_prefix.. of each item; rows 0..n_prefix-1 are copied from `prefix`.
  *   pixels f32 [B, C, img, img]; w f16 [H, kpad] (Conv2d weight flattened [H, C*P*P], zero-padded to
  *   kpad = roundup(C*P*P, 8)); bias f32 [H]; pos f32 [S, H] with S = (img/P)^2 + n_prefix;
@@ -312,7 +312,7 @@ int pe_hop_recv(pe_hop* hop, void* const* ptrs, const size_t* bytes, void* const
 
 /* ---- Debug / bring-up ------------------------------------------------------------------------
  * Reference GEMM on CUDA cores (fp16 inputs, fp32 accumulate, same epilogues). Used ONLY by tests to
- * localise a failure to the tcgen05 kernel; never selected by the product path. */
+ * localise a failure to the wgmma kernel; never selected by the product path. */
 int pe_debug_linear_simt(const void* a, const void* w, const void* bias, const void* resid, void* out, int m, int n,
                          int k, int epilogue, void* stream);
 

@@ -1,7 +1,7 @@
 """Model configurations and default parameters - drop-in for the reference `model_cfg.py`.
 
 Same registry names, layer counts and default weight-file names (`model_cfg.py:23-43`); the `shard_module`
-entries point at the B200 shard classes, and `get_model_config` builds the HuggingFace config from the
+entries point at the native shard classes, and `get_model_config` builds the HuggingFace config from the
 architecture table in `pipeedge_b200.synth` instead of `AutoConfig.from_pretrained` (no network).
 """
 import logging

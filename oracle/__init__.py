@@ -23,8 +23,7 @@ Pinning
 -------
 The reference repo holds no golden vectors for the model path and only a round-trip property test
 for quantisation (`test/quant/test_quant.py:7-30`). The oracle is therefore pinned against the
-reference ITSELF executed in the build container: `oracle/make_goldens.py` imports
-`/root/reference/src/pipeedge` read-only, runs its shard classes and quantisation functions on
+reference ITSELF: `oracle/make_goldens.py` imports a checkout of it (`PIPEEDGE_REFERENCE`, `src/pipeedge`) read-only, runs its shard classes and quantisation functions on
 seeded inputs and writes `tests/golden/*.npz`; `tests/test_oracle_golden.py` (CPU) checks the oracle
 against those fixtures and `tests/test_*_gpu.py` check the CUDA path against both.
 

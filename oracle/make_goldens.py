@@ -1,9 +1,9 @@
 """Generate `tests/golden/*.npz` by executing the REFERENCE itself - TEST INFRASTRUCTURE.
 
-Run in the build container only (`python -m oracle.make_goldens`): imports
-`/root/reference/src/pipeedge` read-only, runs the reference's shard classes and quantisation
-functions on seeded synthetic inputs, and stores the outputs. `/root/reference` does not exist on
-the GPU box, so the fixtures (not this script) are what travels.
+Run where a checkout of the reference (usc-isi/PipeEdge) exists:
+`PIPEEDGE_REFERENCE=<checkout> python -m oracle.make_goldens`. Imports `<checkout>/src/pipeedge` read-only, runs
+the reference's shard classes and quantisation functions on seeded synthetic inputs, and stores the outputs. The
+tests only read the fixtures, never the reference.
 
 Fixture contents
 ----------------
@@ -15,7 +15,7 @@ Fixture contents
   several bit widths, plus the two runtime hooks' clamp thresholds (restated in this script
   without the `monitoring` calls - `runtime.py` itself cannot be imported here, SURVEY.md 8c).
 * `adaptive.json` (`python -m oracle.make_goldens adaptive`): outputs of the reference's adaptive-QuantPipe policy
-  code (`/root/reference/utils/{quant,controller}.py`): `constrain_max_bitwidth` over a grid, Kalman-filter and
+  code (`<checkout>/utils/{quant,controller}.py`): `constrain_max_bitwidth` over a grid, Kalman-filter and
   bit-width-controller traces for fixed measurement sequences.
 """
 import os
@@ -23,7 +23,8 @@ import sys
 import numpy as np
 import torch
 
-REF_SRC = '/root/reference/src'
+REF_ROOT = os.environ.get('PIPEEDGE_REFERENCE', '')   # a checkout of the reference
+REF_SRC = os.path.join(REF_ROOT, 'src')
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 OUT = os.path.join(ROOT, 'tests', 'golden')
 SAMPLE_STRIDE = 97   # prime, so the sample walks across rows and columns
@@ -137,7 +138,7 @@ def _ref_utils():
     """The reference's top-level `utils` package, imported under another name (this repo has its own `utils`)."""
     import importlib.util   # pylint: disable=import-outside-toplevel
     sys.path.insert(0, REF_SRC)   # `utils/quant.py` imports pipeedge.quantization.basic_op
-    pkg_dir = '/root/reference/utils'
+    pkg_dir = os.path.join(REF_ROOT, 'utils')
     spec = importlib.util.spec_from_file_location('ref_utils', os.path.join(pkg_dir, '__init__.py'),
                                                   submodule_search_locations=[pkg_dir])
     pkg = importlib.util.module_from_spec(spec)
@@ -204,7 +205,7 @@ def golden_sched():
     import json   # pylint: disable=import-outside-toplevel
     import logging   # pylint: disable=import-outside-toplevel
     import yaml   # pylint: disable=import-outside-toplevel
-    with open('/root/reference/runtime.py', encoding='utf8') as f:
+    with open(os.path.join(REF_ROOT, 'runtime.py'), encoding='utf8') as f:
         tree = ast.parse(f.read())
     fn = next(n for n in tree.body if isinstance(n, ast.FunctionDef) and n.name == 'parse_yaml_sched')
     from typing import List, Optional, Tuple   # pylint: disable=import-outside-toplevel
@@ -236,6 +237,8 @@ def golden_sched():
 
 
 def main():
+    if not os.path.isdir(os.path.join(REF_SRC, 'pipeedge')):
+        raise SystemExit("set PIPEEDGE_REFERENCE to a checkout of the reference (it must contain src/pipeedge)")
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(8)
     if sys.argv[1:] == ['adaptive']:

@@ -1,7 +1,7 @@
 """ctypes binding of `libpipeedge_b200.so` (the C-ABI declared in `include/pipeedge_b200.h`).
 
 There is no CPU fallback: if the library is missing this module raises at import, and every call on a
-machine without an sm_100 GPU fails with `PipeEdgeB200Error` (PE_ERR_DEVICE).
+machine without an sm_90 (H100) GPU fails with `PipeEdgeB200Error` (PE_ERR_DEVICE).
 """
 import ctypes
 import os

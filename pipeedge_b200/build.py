@@ -1,7 +1,7 @@
-"""Build `libpipeedge_b200.so` (the C-ABI library) in-tree with nvcc for sm_100a.
+"""Build `libpipeedge_b200.so` (the C-ABI library) in-tree with nvcc for sm_90a (H100).
 
-`python -m pipeedge_b200.build` or `__graft_entry__.build()`. The `.so` is git-ignored but travels to
-the GPU box with the snapshot; nothing is JIT-compiled at import time.
+`python -m pipeedge_b200.build` or `__graft_entry__.build()`. The `.so` and the objects are git-ignored build
+products; nothing is JIT-compiled at import time.
 """
 import os
 import subprocess
@@ -12,11 +12,11 @@ PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG_DIR, 'csrc')
 OBJ_DIR = os.path.join(CSRC, 'build')
 LIB_PATH = os.path.join(PKG_DIR, 'libpipeedge_b200.so')
-SOURCES = ['api.cu', 'gemm_tcgen05.cu', 'layernorm.cu', 'attention.cu', 'attention_tcgen05.cu', 'quant.cu', 'stage.cu', 'edges.cu', 'hop.cu', 'link.cu', 'pipe.cu']
+SOURCES = ['api.cu', 'gemm_wgmma.cu', 'layernorm.cu', 'attention.cu', 'attention_wgmma.cu', 'quant.cu', 'stage.cu', 'edges.cu', 'hop.cu', 'link.cu', 'pipe.cu']
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
 # -fmad=false is NOT set globally: the quantisation kernels use explicit _rn intrinsics where bit-exactness
 # matters, everything else may contract.
-FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-std=c++17', '-lineinfo',
+FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-std=c++17', '-lineinfo',
          '-Xcompiler', '-fPIC', '-Xcompiler', '-Wall', '--expt-relaxed-constexpr']
 
 
@@ -42,7 +42,7 @@ def _compile(name: str, verbose: bool) -> str:
 
 
 def build(verbose: bool = False, force: bool = False) -> str:
-    """Compile every CUDA source for sm_100a and link the shared library; returns its path."""
+    """Compile every CUDA source for sm_90a and link the shared library; returns its path."""
     os.makedirs(OBJ_DIR, exist_ok=True)
     sources = [s for s in SOURCES if os.path.exists(os.path.join(CSRC, s))]
     if force:
@@ -53,7 +53,7 @@ def build(verbose: bool = False, force: bool = False) -> str:
     with ThreadPoolExecutor(max_workers=min(8, len(sources))) as pool:
         objs = list(pool.map(lambda s: _compile(s, verbose), sources))
     if force or not os.path.exists(LIB_PATH) or any(os.path.getmtime(o) > os.path.getmtime(LIB_PATH) for o in objs):
-        cmd = [NVCC, '-shared', '-o', LIB_PATH, *objs, '-gencode', 'arch=compute_100a,code=sm_100a', '-lcudart_static',
+        cmd = [NVCC, '-shared', '-o', LIB_PATH, *objs, '-gencode', 'arch=compute_90a,code=sm_90a', '-lcudart_static',
                '-ldl', '-lpthread', '-lrt']
         res = subprocess.run(cmd, capture_output=True, text=True, check=False)
         if res.returncode != 0:

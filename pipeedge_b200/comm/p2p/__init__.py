@@ -2,7 +2,7 @@
 
 Same classes and call contract (`DistP2pContext`, `DistP2pPipelineStage` with `enqueue_tensor`, the four
 `register_*_hook`s, `work_cb` / `results_cb`, FIFO per hop, back-pressure through size-1 queues), rebuilt
-for one rank per B200:
+for one rank per GPU:
 
 * Per-payload control data (the payload description, only when it changes, and any CPU tensors) goes over one
   Unix-domain socket per hop: a Gloo message costs ~170 us of host time (measured), a local socket ~10 us, and at
@@ -822,7 +822,7 @@ class DistP2pPipelineStage:
 
     # ------------------------------------------------------------------ native pipeline selection
     def _native_capable(self) -> bool:
-        """Whether THIS rank's role can run on the native pipeline (csrc/pipe.cu): a B200 shard as the worker, hooks
+        """Whether THIS rank's role can run on the native pipeline (csrc/pipe.cu): a native shard as the worker, hooks
         that the link kernels account for, the reference's ring topology with the data rank on the first stage."""
         rank_src, rank_dst, work_cb, results_cb = self._args
         if os.environ.get('PIPEEDGE_NATIVE', '1') == '0' or not torch.cuda.is_available():
@@ -876,7 +876,7 @@ class DistP2pPipelineStage:
             self._threads['recv'] = TensorRecvThread(queue_in, rank_src)
 
     def init(self) -> None:
-        """Start the threads - or, when every rank runs a B200 shard with hooks the link kernels account for, the
+        """Start the threads - or, when every rank runs a native shard with hooks the link kernels account for, the
         native pipeline (one CUDA graph per micro-batch, stage loop in C; `_native.py`)."""
         assert not self._initialized
         self._initialized = True

@@ -1,4 +1,4 @@
-"""Native pipeline stage: the body of `DistP2pPipelineStage` when every rank drives a B200 shard.
+"""Native pipeline stage: the body of `DistP2pPipelineStage` when every rank drives a native shard.
 
 The reference's stage is three Python threads handing each micro-batch through queues (`p2p/__init__.py:261-295,
 373-394`). Here a stage's micro-batch is ONE CUDA graph (link get -> shard kernels -> link put, `csrc/pipe.cu`) and the
@@ -61,7 +61,7 @@ def hook_is_native(hook) -> bool:
 
 
 def shard_is_native(shard) -> bool:
-    """A B200 shard whose registered hooks the native pipeline accounts for."""
+    """A native shard whose registered hooks the native pipeline accounts for."""
     from ...models.transformers._shard import GpuTransformerShard   # pylint: disable=import-outside-toplevel
     if not isinstance(shard, GpuTransformerShard):
         return False

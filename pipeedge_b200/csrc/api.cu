@@ -40,8 +40,8 @@ bool pdl_enabled() {
 void count_launches(int n) { g_launches.fetch_add(static_cast<uint64_t>(n), std::memory_order_relaxed); }
 uint64_t launch_count_now() { return g_launches.load(std::memory_order_relaxed); }
 
-// The kernels use tcgen05 / TMEM / TMA PTX that exists only on sm_100: refuse anything else loudly.
-int require_sm100() {
+// The library is built for sm_90a only (wgmma / TMA / cluster PTX, compute capability 9.0): refuse anything else loudly.
+int require_sm90() {
   static int cached = 1;  // 1 = unknown
   if (cached == 1) {
     int dev = 0, major = 0;
@@ -51,8 +51,8 @@ int require_sm100() {
       cudaGetLastError();
       return PE_ERR_DEVICE;
     }
-    if (major != 10) {
-      set_error("device compute capability major %d is not 10 (sm_100a required)", major);
+    if (major != 9) {
+      set_error("device compute capability major %d is not 9 (sm_90a required)", major);
       return PE_ERR_DEVICE;
     }
     cached = PE_OK;
@@ -95,7 +95,7 @@ uint64_t pe_launch_count(void) { return pe::g_launches.load(std::memory_order_re
 
 int pe_layernorm(const void* x, const void* gamma, const void* beta, float eps, void* out_f32, void* out_f16, int rows,
                  int hidden, void* stream) {
-  int rc = pe::require_sm100();
+  int rc = pe::require_sm90();
   if (rc != PE_OK) return rc;
   return pe::layernorm_impl(x, nullptr, gamma, beta, eps, nullptr, out_f32, out_f16, rows, hidden,
                             static_cast<cudaStream_t>(stream));
@@ -103,7 +103,7 @@ int pe_layernorm(const void* x, const void* gamma, const void* beta, float eps, 
 
 int pe_residual_layernorm(const void* y, const void* resid, const void* gamma, const void* beta, float eps,
                           void* sum_out, void* out_f32, void* out_f16, int rows, int hidden, void* stream) {
-  int rc = pe::require_sm100();
+  int rc = pe::require_sm90();
   if (rc != PE_OK) return rc;
   return pe::layernorm_impl(y, resid, gamma, beta, eps, sum_out, out_f32, out_f16, rows, hidden,
                             static_cast<cudaStream_t>(stream));
@@ -126,7 +126,7 @@ int pe_linear_ln_cluster(int n) { return pe::linear_ln_cluster(n); }
 
 int pe_debug_linear_simt(const void* a, const void* w, const void* bias, const void* resid, void* out, int m, int n,
                          int k, int epilogue, void* stream) {
-  int rc = pe::require_sm100();
+  int rc = pe::require_sm90();
   if (rc != PE_OK) return rc;
   return pe::linear_simt_impl(a, w, bias, resid, out, m, n, k, epilogue, static_cast<cudaStream_t>(stream));
 }
@@ -139,19 +139,19 @@ int pe_debug_gemm_trace(void* buf) {
 int pe_debug_gemm_plan(int m, int n, int k, int epilogue, int* out6) { return pe::gemm_plan_query(m, n, k, epilogue, out6); }
 
 int pe_attention(const void* qkv, void* ctx, int batch, int tokens, int heads, int head_dim, void* stream) {
-  int rc = pe::require_sm100();
+  int rc = pe::require_sm90();
   if (rc != PE_OK) return rc;
   return pe::attention_impl(qkv, ctx, batch, tokens, heads, head_dim, static_cast<cudaStream_t>(stream));
 }
 
 int pe_cast_f32_to_f16(const void* src, void* dst, size_t n, void* stream) {
-  int rc = pe::require_sm100();
+  int rc = pe::require_sm90();
   if (rc != PE_OK) return rc;
   return pe::cast_impl(src, dst, n, true, static_cast<cudaStream_t>(stream));
 }
 
 int pe_cast_f16_to_f32(const void* src, void* dst, size_t n, void* stream) {
-  int rc = pe::require_sm100();
+  int rc = pe::require_sm90();
   if (rc != PE_OK) return rc;
   return pe::cast_impl(src, dst, n, false, static_cast<cudaStream_t>(stream));
 }
@@ -162,7 +162,7 @@ float pe_quant_clamp_factor(int bit, int gelu) { return pe::clamp_factor(bit, ge
 
 int pe_quant_encode(const void* x, int items, size_t n, int bit, int clamp, void* codes, void* scale, void* shift,
                     void* alpha, void* work, void* stream) {
-  int rc = pe::require_sm100();
+  int rc = pe::require_sm90();
   if (rc != PE_OK) return rc;
   return pe::quant_encode_impl(x, items, n, bit, clamp, codes, scale, shift, alpha, work,
                                static_cast<cudaStream_t>(stream));
@@ -170,14 +170,14 @@ int pe_quant_encode(const void* x, int items, size_t n, int bit, int clamp, void
 
 int pe_quant_alpha(const void* x, int items, size_t n, int bit, int clamp, void* scale, void* shift, void* alpha,
                    void* work, void* stream) {
-  int rc = pe::require_sm100();
+  int rc = pe::require_sm90();
   if (rc != PE_OK) return rc;
   return pe::quant_stats_impl(x, items, n, bit, clamp, scale, shift, alpha, work, static_cast<cudaStream_t>(stream));
 }
 
 int pe_quant_decode(const void* codes, int items, size_t n, int bit, const void* scale, const void* shift, void* out,
                     void* stream) {
-  int rc = pe::require_sm100();
+  int rc = pe::require_sm90();
   if (rc != PE_OK) return rc;
   return pe::quant_decode_impl(codes, items, n, bit, scale, shift, out, static_cast<cudaStream_t>(stream));
 }

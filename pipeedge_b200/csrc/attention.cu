@@ -7,8 +7,9 @@
 // scale folded in); P is rounded to fp16 for the P.V product, accumulators stay fp32 in registers. The number
 // of warps per CTA and of query splits is picked so that S = 197 wastes < 6 % of the rows (13 row groups ->
 // 2 CTAs of 7 warps) instead of padding to 256.
-// Round-1 version on the warp-level tensor-core path (mma.sync m16n8k16); attention is ~4% of the
-// block's FLOPs (SURVEY.md 8d). Replaces HF eager_attention_forward (see pe_attention in the header).
+// Tensor cores through the warp-level mma.sync m16n8k16 path: the fall-back for the shapes the wgmma kernel
+// (attention_wgmma.cu) does not take - head_dim 80, S > 256 - and the kernel PE_ATTN_WGMMA=0 selects. Attention is
+// ~4% of the block's FLOPs (SURVEY.md 8d). Replaces HF eager_attention_forward (see pe_attention in the header).
 #include <cstdlib>
 
 #include "../../include/pipeedge_b200.h"
@@ -17,8 +18,8 @@
 namespace pe {
 
 void count_launches(int n);
-int attention_tcgen05_impl(const void* qkv, void* ctx, int batch, int tokens, int heads, int head_dim,
-                           cudaStream_t stream);
+int attention_wgmma_impl(const void* qkv, void* ctx, int batch, int tokens, int heads, int head_dim,
+                         cudaStream_t stream);
 
 constexpr int kAttnKc = 64;
 constexpr int kAttnMaxWarps = 8;
@@ -249,7 +250,7 @@ attention_kernel(const __half* __restrict__ qkv, __half* __restrict__ ctx, int t
 template <int kAttnD>
 static int launch_attention(const void* qkv, void* ctx, int batch, int tokens, int heads, cudaStream_t stream) {
   // 16-row groups -> query splits of at most 8 warps; prefer the fewest splits (K/V are staged once per CTA)
-  // that still give the 148 SMs a full wave of CTAs
+  // that still give the SMs a full wave of CTAs
   const int groups = (tokens + 15) / 16;
   int splits = (groups + kAttnMaxWarps - 1) / kAttnMaxWarps;
   while (static_cast<long>(splits) * heads * batch < kNumSMs && splits < groups) ++splits;
@@ -279,12 +280,12 @@ static int launch_attention(const void* qkv, void* ctx, int batch, int tokens, i
 int attention_impl(const void* qkv, void* ctx, int batch, int tokens, int heads, int head_dim, cudaStream_t stream) {
   PE_REQUIRE(qkv && ctx, "pe_attention: null pointer");
   PE_REQUIRE(batch > 0 && tokens > 0 && heads > 0, "pe_attention: bad shape");
-  static const int use_tcgen05 = [] {
-    const char* e = getenv("PE_ATTN_TCGEN05");
-    return (e != nullptr && e[0] == '0') ? 0 : 1;     // PE_ATTN_TCGEN05=0 selects the mma.sync kernel below
+  static const int use_wgmma = [] {
+    const char* e = getenv("PE_ATTN_WGMMA");
+    return (e != nullptr && e[0] == '0') ? 0 : 1;     // PE_ATTN_WGMMA=0 selects the mma.sync kernel below
   }();
-  if (use_tcgen05) {   // shapes the tcgen05 kernel does not take (head_dim != 64, S > 256) fall through
-    const int rc = attention_tcgen05_impl(qkv, ctx, batch, tokens, heads, head_dim, stream);
+  if (use_wgmma) {   // shapes the wgmma kernel does not take (head_dim != 64, S > 256) fall through
+    const int rc = attention_wgmma_impl(qkv, ctx, batch, tokens, heads, head_dim, stream);
     if (rc != PE_ERR_INVALID) return rc;
   }
   if (head_dim == 64) return launch_attention<64>(qkv, ctx, batch, tokens, heads, stream);

@@ -1,4 +1,4 @@
-// Shared device helpers for the sm_100a kernels: mbarrier, TMA, tcgen05/TMEM PTX wrappers,
+// Shared device helpers for the sm_90a kernels: mbarrier, TMA, clusters, wgmma synchronisation and descriptors,
 // warp reductions and the status/error plumbing of the C-ABI.
 #pragma once
 #include <cuda.h>
@@ -25,7 +25,7 @@ int check_cuda(cudaError_t err, const char* what);
     }                                                  \
   } while (0)
 
-constexpr int kNumSMs = 148;  // B200
+constexpr int kNumSMs = 132;  // H100 SXM
 
 // ---------------------------------------------------------------- small utilities
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -48,7 +48,7 @@ __device__ __forceinline__ float warp_max(float v) {
 
 // ---------------------------------------------------------------- programmatic dependent launch (PDL)
 // Every kernel of the stage path is launched with programmatic stream serialisation: it may become resident while
-// its predecessor is still draining, runs its private prologue (barrier init, TMEM alloc, descriptor prefetch) and then
+// its predecessor is still draining, runs its private prologue (barrier init, descriptor prefetch) and then
 // blocks in pdl_wait() until the predecessor has completed and its writes are visible. Rules (stage.cu relies on them):
 // no global read of produced data and no global write before pdl_wait(); every PDL-launched kernel calls pdl_wait()
 // on every thread that touches global memory, so completion stays transitive along the stream.
@@ -91,47 +91,6 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
                : "memory");
 }
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-// Bounded wait: a protocol bug must end in a trap (the launch fails, the caller sees an error) rather
-// than hang the GPU. ~2^31 cycles is about a second at B200 clocks; real waits are microseconds.
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  if (mbar_try_wait(bar, parity)) return;
-  const long long t0 = clock64();
-  while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > (1ll << 31)) {
-      printf("pipeedge_b200: mbarrier wait timed out (block %d thread %d)\n", blockIdx.x, threadIdx.x);
-      __trap();
-    }
-  }
-}
-
-// Long waits (an epilogue warp waiting for a whole main loop): back off with nanosleep so that the spinning
-// warp does not take issue slots from the single-thread TMA / MMA roles sharing its scheduler (the r01
-// kernels lost ~650 cycles per K block to exactly that: the arbiter favours higher warp ids).
-__device__ __forceinline__ void mbar_wait_relaxed(uint64_t* bar, uint32_t parity) {
-  if (mbar_try_wait(bar, parity)) return;
-  const long long t0 = clock64();
-  unsigned ns = 32;
-  while (!mbar_try_wait(bar, parity)) {
-    __nanosleep(ns);
-    if (ns < 256) ns <<= 1;
-    if (clock64() - t0 > (1ll << 31)) {
-      printf("pipeedge_b200: mbarrier wait timed out (block %d thread %d)\n", blockIdx.x, threadIdx.x);
-      __trap();
-    }
-  }
-}
-
 // ---- lean variants for the single-issuer hot loops: 32-bit shared addresses computed once, the spin lives in
 // PTX (a handful of instructions per retry). A lone warp issues roughly one dependent instruction every 6-8
 // cycles, so every instruction in those loops costs as much as ~1/64 of a 128x256x64 MMA block.
@@ -198,31 +157,6 @@ __device__ __forceinline__ void tma_load_2d_multicast_addr(uint32_t smem_dst, co
       ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar_addr), "r"(c0), "r"(c1), "h"(cta_mask)
       : "memory");
 }
-// tcgen05.mma with the 64-bit shared-memory descriptors assembled in PTX from their 32-bit halves
-__device__ __forceinline__ void umma_f16_ss_lohi(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo, uint32_t desc_hi,
-                                                 uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %3};\n\t"
-      "mov.b64 db, {%2, %3};\n\t"
-      "setp.ne.b32 p, %5, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, p;\n\t}"
-      ::"r"(tmem_d), "r"(a_lo), "r"(b_lo), "r"(desc_hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_addr(uint32_t bar_addr) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar_addr) : "memory");
-}
-__device__ __forceinline__ void umma_commit_multicast_addr(uint32_t bar_addr, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(bar_addr), "h"(cta_mask)
-      : "memory");
-}
-// halves of the K-major SWIZZLE_128B descriptor (see umma_desc_kmajor_sw128)
-__device__ __forceinline__ uint32_t umma_desc_lo(uint32_t smem_addr) { return ((smem_addr & 0x3FFFFu) >> 4) | (1u << 16); }
-constexpr uint32_t kUmmaDescHiSw128 = (1024u >> 4) | (1u << 14) | (2u << 29);
-
 // ---------------------------------------------------------------- TMA
 // Pull one box of a tensor into L2 without a shared-memory destination (weights ahead of their first use).
 __device__ __forceinline__ void tma_prefetch_l2_2d(const CUtensorMap* map, int c0, int c1) {
@@ -293,25 +227,21 @@ __device__ __forceinline__ float2 ld_dsmem_f2(uint32_t cluster_addr) {
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_bar_addr) {
   asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar_addr) : "memory");
 }
-// wait on this CTA's mbarrier with cluster-scope acquire (pairs with mbar_arrive_cluster); bounded like mbar_wait
+// wait on this CTA's mbarrier with cluster-scope acquire (pairs with mbar_arrive_cluster); bounded like mbar_wait_addr
+// and without a printf, which would be a function call that serialises the caller's wgmma pipeline
 __device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-  const uint32_t addr = smem_u32(bar);
-  const long long t0 = clock64();
-  for (;;) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(addr), "r"(parity)
-        : "memory");
-    if (ok) return;
-    if (clock64() - t0 > (1ll << 31)) {
-      printf("pipeedge_b200: cluster mbarrier wait timed out (block %d thread %d)\n", blockIdx.x, threadIdx.x);
-      __trap();
-    }
-  }
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t.reg .u32 n;\n\tmov.u32 n, 0;\n"
+      "PE_WAITC:\n\t"
+      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%0], %1;\n\t"
+      "@p bra PE_DONEC;\n\t"
+      "add.u32 n, n, 1;\n\t"
+      "setp.lt.u32 p, n, 16777216;\n\t"
+      "@p bra PE_WAITC;\n\t"
+      "trap;\n"
+      "PE_DONEC:\n\t}"
+      ::"r"(smem_u32(bar)), "r"(parity)
+      : "memory");
 }
 // named barrier among `threads` threads of the CTA (ids 1..15; 0 is __syncthreads)
 template <int kId>
@@ -319,93 +249,25 @@ __device__ __forceinline__ void named_barrier(int threads) {
   asm volatile("bar.sync %0, %1;" ::"n"(kId), "r"(threads) : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread on behalf of the CTA.
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on `bar` once every tcgen05.mma issued so far by this thread has completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// Same, arriving on the barrier at this CTA-relative offset in every CTA of `cta_mask`.
-__device__ __forceinline__ void umma_commit_multicast(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"(cta_mask)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// 32 lanes x 16 consecutive fp32 columns: thread t of the warp gets row (lane base + t).
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32"
-      " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
+// ---------------------------------------------------------------- wgmma (warpgroup MMA)
+// Order this thread's earlier register / shared-memory accesses before the wgmma instructions that follow.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// wait until at most N of this warpgroup's committed wgmma groups are still in flight
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// 32 lanes x 32 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32"
-      " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
-      " %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-
-// Shared-memory matrix descriptor for a K-major fp16 tile stored as rows of 128 bytes with the
-// 128-byte swizzle (what a TMA box of 64 fp16 x R rows with CU_TENSOR_MAP_SWIZZLE_128B writes):
-// 8-row groups are 1024 bytes apart (SBO); LBO is unused for swizzled K-major layouts.
-// Field layout follows the PTX ISA "matrix descriptor" for tcgen05 (version field = 1).
-__device__ __forceinline__ uint64_t umma_desc_kmajor_sw128(uint32_t smem_addr) {
+// Shared-memory matrix descriptor for a K-major fp16 tile stored as rows of 128 bytes with the 128-byte swizzle (what a
+// TMA box of 64 fp16 x R rows with CU_TENSOR_MAP_SWIZZLE_128B writes): 8-row groups are 1024 bytes apart (SBO); LBO is
+// unused for swizzled K-major layouts. Field layout of the PTX ISA wgmma matrix descriptor; the tile must start on a
+// 1024-byte boundary (base offset 0). Advancing K by 16 fp16 inside the swizzled row adds 32 bytes to the start address.
+__device__ __forceinline__ uint64_t wgmma_desc_kmajor_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);  // start address  [0,14)
   d |= static_cast<uint64_t>(1) << 16;                      // LBO (ignored)  [16,30)
   d |= static_cast<uint64_t>(1024 >> 4) << 32;              // SBO = 1024 B   [32,46)
-  d |= static_cast<uint64_t>(1) << 46;                      // version = 1    [46,48)
-  d |= static_cast<uint64_t>(2) << 61;                      // SWIZZLE_128B   [61,64)
+  d |= static_cast<uint64_t>(1) << 62;                      // SWIZZLE_128B   [62,64)
   return d;
-}
-// Instruction descriptor, kind::f16: fp16 A and B (both K-major), fp32 accumulate, M x N tile.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int m, int n) {
-  return (1u << 4)                                   // D format = F32
-         | (0u << 7) | (0u << 10)                    // A, B format = F16
-         | (0u << 15) | (0u << 16)                   // A, B K-major
-         | (static_cast<uint32_t>(n >> 3) << 17)     // N / 8
-         | (static_cast<uint32_t>(m >> 4) << 24);    // M / 16
 }
 
 }  // namespace pe

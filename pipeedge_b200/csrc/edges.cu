@@ -1,5 +1,5 @@
 // Stage-0 edges of the pipeline (SURVEY.md 8a-A13): patch embedding for ViT/DeiT and the BERT embedding
-// gather + LayerNorm. Small, HBM-bound kernels around one tcgen05 GEMM.
+// gather + LayerNorm. Small, HBM-bound kernels around one wgmma GEMM.
 //   ViT/DeiT: HF ViTEmbeddings/DeiTEmbeddings = Conv2d(C, H, P, stride P) -> flatten -> [CLS (, DIST)] ++ patches, + pos.
 //             The strided conv is a GEMM over im2col'ed patches: [B*Np, C*P*P] x [H, C*P*P]^T; its epilogue adds
 //             the conv bias and the position rows and scatters into token rows n_prefix.. of each item.
@@ -10,7 +10,7 @@
 namespace pe {
 
 void count_launches(int n);
-int require_sm100();
+int require_sm90();
 int linear_impl(const void* a, const void* w, const void* bias, const void* resid, void* out, int m, int n, int k,
                 int epilogue, int rows_per_item, int out_item_rows, int out_row_offset, int resid_per_item,
                 int static_w, cudaStream_t stream);
@@ -116,7 +116,7 @@ int pe_patch_embed(const void* pixels, const void* w, const void* bias, const vo
   PE_REQUIRE(pixels && w && bias && pos && prefix && out && patches_work, "pe_patch_embed: null pointer");
   PE_REQUIRE(batch > 0 && channels > 0 && patch > 0 && img % patch == 0 && hidden % 8 == 0 && n_prefix >= 1,
              "pe_patch_embed: bad shape");
-  int rc = require_sm100();
+  int rc = require_sm90();
   if (rc != PE_OK) return rc;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   const int np_side = img / patch, np = np_side * np_side;
@@ -145,7 +145,7 @@ int pe_bert_embed(const void* ids, const void* pos_ids, const void* word, const 
   using namespace pe;
   PE_REQUIRE(ids && pos_ids && word && type0 && pos && gamma && beta && out, "pe_bert_embed: null pointer");
   PE_REQUIRE(batch > 0 && seq > 0 && hidden % 4 == 0 && hidden <= kEmbMaxVec * 128, "pe_bert_embed: bad shape");
-  int rc = require_sm100();
+  int rc = require_sm90();
   if (rc != PE_OK) return rc;
   const int rows = batch * seq;
   bert_embed_kernel<<<(rows + 3) / 4, 128, 0, static_cast<cudaStream_t>(stream_v)>>>(

@@ -23,7 +23,7 @@
 
 namespace pe {
 
-int require_sm100();
+int require_sm90();
 
 // minimal NCCL surface (ABI-stable since NCCL 2.x)
 typedef struct ncclComm* ncclComm_t;
@@ -130,7 +130,7 @@ int pe_hop_available(void) { return pe::nccl().ok ? 1 : 0; }
 int pe_hop_open(int fd, int is_sender, pe_hop** out) {
   using namespace pe;
   PE_REQUIRE(out != nullptr && fd >= 0, "pe_hop_open: bad arguments");
-  int rc = require_sm100();
+  int rc = require_sm90();
   if (rc != PE_OK) return rc;
   NcclApi& api = nccl();
   PE_REQUIRE(api.ok, "pe_hop_open: libnccl.so.2 is not loadable in this process");

@@ -37,7 +37,7 @@
 namespace pe {
 
 void count_launches(int n);
-int require_sm100();
+int require_sm90();
 float clamp_factor(int bit, int gelu);
 size_t quant_words(size_t n, int bit);
 size_t quant_workspace_bytes(int items, size_t n);
@@ -724,8 +724,8 @@ static int alloc_common(pe_link* l) {
   const char* w = getenv("PIPEEDGE_WIRE_F16");
   l->wire_f16 = (w != nullptr && w[0] == '1') ? 1 : 0;
   // Default 2: one GPU-scope fence per CTA, one system-scope fence by the CTA that publishes the slot (the release is
-  // cumulative over what the arrival counter ordered before it). A system-scope fence in every CTA cost 12 us per
-  // send + receive pair of a 4.8 MB payload (profiles/r02_link_bench.txt); PE_LINK_SYNC=0 restores it.
+  // cumulative over what the arrival counter ordered before it): a system-scope fence in every CTA makes each CTA wait
+  // for its stores to become visible system-wide. PE_LINK_SYNC=0 restores that stricter mode.
   const char* sm = getenv("PE_LINK_SYNC");
   l->sync_mode = sm != nullptr ? atoi(sm) : 2;
   const char* gc = getenv("PE_LINK_GRID_CAP");
@@ -1041,7 +1041,7 @@ extern "C" {
 int pe_link_open(int fd, int is_producer, size_t slot_payload_bytes, int n_slots, int quant_hint, pe_link** out) {
   using namespace pe;
   PE_REQUIRE(out != nullptr && fd >= 0, "pe_link_open: bad arguments");
-  int rc = require_sm100();
+  int rc = require_sm90();
   if (rc != PE_OK) return rc;
   pe_link* l = new pe_link();
   l->fd = fd;
@@ -1136,7 +1136,7 @@ int pe_link_open_local(size_t slot_payload_bytes, int n_slots, int quant_hint, p
   using namespace pe;
   PE_REQUIRE(out != nullptr && n_slots >= 2 && n_slots <= kLinkMaxSlots && slot_payload_bytes > 0,
              "pe_link_open_local: bad arguments");
-  int rc = require_sm100();
+  int rc = require_sm90();
   if (rc != PE_OK) return rc;
   pe_link* l = new pe_link();
   l->kind = 1;
@@ -1185,7 +1185,7 @@ int pe_link_open_host(size_t slot_payload_bytes, int n_slots, pe_link** out) {
   using namespace pe;
   PE_REQUIRE(out != nullptr && n_slots >= 2 && n_slots <= kLinkMaxSlots && slot_payload_bytes > 0,
              "pe_link_open_host: bad arguments");
-  int rc = require_sm100();
+  int rc = require_sm90();
   if (rc != PE_OK) return rc;
   pe_link* l = new pe_link();
   l->kind = 2;

@@ -1,4 +1,4 @@
-// LayerNorm row statistics shared by the fused projection + residual + LayerNorm epilogue (gemm_tcgen05.cu) and the
+// LayerNorm row statistics shared by the fused projection + residual + LayerNorm epilogue (gemm_wgmma.cu) and the
 // stand-alone kernel that mirrors it (layernorm.cu). A row is cut into 32-column chunks; each chunk is reduced to
 // (mean, M2 = sum of squared deviations) by ONE thread in index order, chunks are merged in column order inside a slice of
 // `slice` columns, slices in column order across the row (Chan's parallel update). Every step is an explicit IEEE

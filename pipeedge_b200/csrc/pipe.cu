@@ -25,7 +25,7 @@
 namespace pe {
 void count_launches(int n);
 uint64_t launch_count_now();
-int require_sm100();
+int require_sm90();
 constexpr int kPipeWindow = 8;   // graph launches the host may run ahead of the device
 }  // namespace pe
 
@@ -143,7 +143,7 @@ int pe_pipe_create(pe_link* in, pe_link* out, pe_link* res, pe_pipe** out_pipe) 
   using namespace pe;
   PE_REQUIRE(out_pipe != nullptr && in != nullptr && out != nullptr, "pe_pipe_create: null link");
   PE_REQUIRE(in->is_rx && out->is_tx && (res == nullptr || res->is_rx), "pe_pipe_create: link ends do not match their roles");
-  int rc = require_sm100();
+  int rc = require_sm90();
   if (rc != PE_OK) return rc;
   pe_pipe* p = new pe_pipe();
   p->in = in;

@@ -22,7 +22,7 @@
 namespace pe {
 
 void count_launches(int n);
-int require_sm100();
+int require_sm90();
 int linear_impl(const void* a, const void* w, const void* bias, const void* resid, void* out, int m, int n, int k,
                 int epilogue, int rows_per_item, int out_item_rows, int out_row_offset, int resid_per_item,
                 int static_w, cudaStream_t stream);
@@ -124,7 +124,7 @@ static int enqueue(pe_stage* st, const void* in0, const void* in1, void* out0, v
   bool pending = false;         // residual stream = t32 + skip, not yet added (pre-LN only)
   bool a16_valid = false;       // a16 holds the f16 copy of x (post-LN only)
 
-  // Projection + residual add + LayerNorm as ONE kernel (cluster epilogue, gemm_tcgen05.cu) wherever the LayerNorm that
+  // Projection + residual add + LayerNorm as ONE kernel (cluster epilogue, gemm_wgmma.cu) wherever the LayerNorm that
   // follows an output projection / FC2 belongs to this stage and the width splits into <= 8 slices of <= 128 columns.
   const bool fuse_ln = fuse_ln_enabled() && linear_ln_cluster(H) > 0;
   bool a16_ready = false;       // pre-LN: a16 already holds LayerNorm(x) for the sub-layer about to run
@@ -269,7 +269,7 @@ int pe_stage_create(const pe_stage_desc* desc, const pe_block_weights* blocks, i
              "pe_stage_create: hidden=%d heads=%d (head_dim must be 64 or 80)", desc->hidden, desc->heads);
   PE_REQUIRE(desc->hidden % 8 == 0 && desc->inter % 8 == 0 && desc->inter > 0, "pe_stage_create: bad hidden/inter");
   PE_REQUIRE(desc->tokens > 0 && desc->max_ubatch > 0, "pe_stage_create: bad tokens/max_ubatch");
-  int rc = require_sm100();
+  int rc = require_sm90();
   if (rc != PE_OK) return rc;
   pe_stage* st = new pe_stage();
   st->d = *desc;

@@ -1,6 +1,6 @@
 """Model shard base types - same public names and semantics as the reference `pipeedge.models`
 (`src/pipeedge/models/__init__.py:1-49`), so reference callers (`runtime.py`, `model_cfg.py`) work
-unchanged against the B200 shards."""
+unchanged against the native shards."""
 from typing import Any, Tuple, Type, Union
 from torch import nn, Tensor
 

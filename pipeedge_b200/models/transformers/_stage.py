@@ -105,7 +105,7 @@ class EncoderStage:
     def __init__(self, family: str, config, layer_start: int, layer_end: int, weights: Mapping, tokens: int,
                  max_ubatch: int = 64):
         if not torch.cuda.is_available():
-            raise RuntimeError("pipeedge_b200 shards need a CUDA (sm_100a) device: there is no CPU fallback")
+            raise RuntimeError("pipeedge_b200 shards need a CUDA (sm_90a) device: there is no CPU fallback")
         self.family = family
         self.hidden = int(config.hidden_size)
         self.heads = int(config.num_attention_heads)

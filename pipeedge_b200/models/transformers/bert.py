@@ -1,4 +1,4 @@
-"""BERT shards on B200 - drop-in for `pipeedge.models.transformers.bert` (reference `bert.py`).
+"""BERT shards on H100 - drop-in for `pipeedge.models.transformers.bert` (reference `bert.py`).
 
 Post-LN blocks (`bert.py:41-52`), no attention mask (`bert.py:45`), HF state_dict `.npz` layout
 (`bert.py:104-140`; the classification shard strips a `bert.` prefix, `bert.py:191-196`). The reference leaves

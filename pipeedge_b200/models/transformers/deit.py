@@ -1,4 +1,4 @@
-"""DeiT shards on B200 - drop-in for `pipeedge.models.transformers.deit` (reference `deit.py`).
+"""DeiT shards on H100 - drop-in for `pipeedge.models.transformers.deit` (reference `deit.py`).
 
 DeiT blocks are ViT blocks (`deit.py:27-69` copies `ViTLayerShard`); what differs is the timm `.npz` key
 layout (`deit.py:119-156`), the extra distillation token (S = 198) and that only the `head` classifier is used

@@ -1,8 +1,8 @@
-"""ViT shards on B200 - drop-in for `pipeedge.models.transformers.vit` (reference `vit.py`).
+"""ViT shards on H100 - drop-in for `pipeedge.models.transformers.vit` (reference `vit.py`).
 
 Same class names, constructor and `forward` contract; the arithmetic (HF `ViTEmbeddings`, `ViTSelfAttention`,
 `ViTSelfOutput`, `ViTIntermediate`, `ViTOutput`, `nn.LayerNorm`, the classifier `nn.Linear`) runs as the
-sm_100a kernels of `libpipeedge_b200.so`. Weights are read from the Google/JAX `.npz` layout the reference
+sm_90a kernels of `libpipeedge_b200.so`. Weights are read from the Google/JAX `.npz` layout the reference
 loads (`vit.py:120-159,216-218`).
 """
 from collections.abc import Mapping

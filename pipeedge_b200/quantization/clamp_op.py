@@ -1,6 +1,6 @@
 """Banner-2019 clamps on the device - drop-in for `pipeedge.quantization.clamp_op` (reference `clamp_op.py`).
 
-The pipeline never calls these directly on the B200 path (the clamp is fused into the encode kernels, see
+The pipeline never calls these directly on the native path (the clamp is fused into the encode kernels, see
 `basic_op.tensor_encode_outerdim(clamp=True)`); they exist for API parity and tests. The threshold comes
 from the library's statistics kernels; only the final elementwise min/max uses torch."""
 import torch

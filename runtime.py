@@ -3,7 +3,7 @@
 Same CLI (`runtime.py:610-687`): `runtime.py RANK WORLDSIZE [-d] [-s] [--addr] [--port] [-c p2p] [-m] [-M] [-b]
 [-u] [-pt] [-q] [-r] [-D]`, same schedule semantics (`-pt` 1-based inclusive sub-layer pairs, `-q` bits per
 stage output, `-r` stage-to-rank order, `-D` data rank), same command protocol (CMD_STOP / CMD_SCHED) and the
-same hook structure around the shard (`run_pipeline_p2p`, `runtime.py:418-511`). One rank per B200:
+same hook structure around the shard (`run_pipeline_p2p`, `runtime.py:418-511`). One rank per GPU:
 activations stay in HBM, the hop is NCCL on a side stream, and the QuantPipe hooks call the fused device
 kernels (bit-identical codes). The adaptive QuantPipe policies (`ADAPTIVE_QUANT=HEURISTIC|HEURISTIC2|CONTROLLER`
 with `SEND_CONSTRAINT` items/s and `WINDOW_SIZE`, `runtime.py:121-216`) are carried over; they read the hop's

@@ -1,4 +1,4 @@
-"""Coefficients of gelu_erf_fast (pipeedge_b200/csrc/gemm_tcgen05.cu): degree-7 fit of log2(erfc(a/sqrt2)/2) on [0, 6]
+"""Coefficients of gelu_erf_fast (pipeedge_b200/csrc/gemm_wgmma.cu): degree-7 fit of log2(erfc(a/sqrt2)/2) on [0, 6]
 at Chebyshev nodes, expanded to the power basis, and its error against the exact erf GELU in emulated fp32."""
 import numpy as np
 from numpy.polynomial import Polynomial, chebyshev as C, polynomial as P

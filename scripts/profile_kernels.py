@@ -1,9 +1,9 @@
 """One launch of every kernel on the hot path at BASELINE shapes, bracketed by cudaProfilerStart/Stop, for
 
-    ncu --set full --clock-control none --import-source on --profile-from-start off -o gpurun_out/.../kernels \
+    ncu --set full --clock-control none --import-source on --profile-from-start off -o kernels \
         python scripts/profile_kernels.py
 
-ViT-B micro-batch 8 (M = 1576): LayerNorm (+ residual), the four tcgen05 GEMMs, attention, patch embedding (im2col + GEMM +
+ViT-B micro-batch 8 (M = 1576): LayerNorm (+ residual), the four wgmma GEMMs, attention, patch embedding (im2col + GEMM +
 prefix rows); BASELINE config 5's hop [32, 198, 768] at 8 bits: the three stand-alone quant kernels, decode, the fused
 quantise-and-send and the receive kernel of a link, the raw send / receive; BERT embedding [32, 128]."""
 import ctypes

@@ -20,9 +20,11 @@ def _env(port):
     os.environ['CUDA_VISIBLE_DEVICES'] = ''   # this suite is the Gloo path
 
 
-def test_context_lifecycle_world1():
+def test_context_lifecycle_world1(monkeypatch):
     from pipeedge_b200.comm.p2p import DistP2pContext
-    _env(_free_port())
+    # runs in the pytest process itself: hiding the GPU here (CUDA_VISIBLE_DEVICES) would hide it from every later test
+    monkeypatch.setenv('MASTER_ADDR', '127.0.0.1')
+    monkeypatch.setenv('MASTER_PORT', str(_free_port()))
     ctx = DistP2pContext(('gloo',), {'world_size': 1, 'rank': 0}, lambda cmd, tensors: None)
     ctx.init()
     ctx.shutdown()

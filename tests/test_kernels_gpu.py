@@ -1,7 +1,7 @@
 """GPU: each kernel of libpipeedge_b200.so, called through the C-ABI, against a plain fp32 restatement.
 
 LayerNorm / GEMM / attention are floating point: compared with torch fp32 maths on the same (fp16-rounded)
-operands, tolerances written in each test. The tcgen05 GEMM is additionally compared with the library's own
+operands, tolerances written in each test. The wgmma GEMM is additionally compared with the library's own
 CUDA-core debug GEMM to localise failures.
 """
 import math
@@ -76,7 +76,7 @@ GEMM_SHAPES = [(128, 256, 64), (128, 128, 128), (256, 512, 768), (1576, 2304, 76
 
 @pytest.mark.parametrize('epi_name', ['PE_EPI_F16', 'PE_EPI_GELU_F16', 'PE_EPI_RESID_F32', 'PE_EPI_F32', 'PE_EPI_TANH_F32'])
 def test_linear_simt_debug_kernel(ops, epi_name):
-    """The CUDA-core debug GEMM itself is right (it is the comparator for the tcgen05 kernel)."""
+    """The CUDA-core debug GEMM itself is right (it is the comparator for the wgmma kernel)."""
     epi = getattr(_lib(), epi_name)
     a, w, bias, resid = _gemm_case(77, 200, 136, 5)
     want = _gemm_ref(a, w, bias, resid, epi)
@@ -146,7 +146,8 @@ def test_linear_rejects_bad_arguments(ops):
 
 
 @pytest.mark.parametrize('batch,tokens,heads', [(2, 197, 12), (1, 128, 2), (3, 17, 2), (1, 64, 1), (1, 65, 1),
-                                                (2, 198, 12), (1, 1, 1), (1, 512, 2), (2, 257, 16)])
+                                                (2, 198, 12), (1, 1, 1), (1, 512, 2), (2, 257, 16), (1, 256, 2),
+                                                (8, 197, 12), (4, 240, 3), (32, 128, 12), (16, 197, 16)])
 @pytest.mark.parametrize('head_dim', [64, 80])
 def test_attention(ops, batch, tokens, heads, head_dim):
     """head_dim 64 (ViT-B/L, DeiT, BERT) and 80 (ViT-Huge)."""
@@ -163,7 +164,8 @@ def test_attention(ops, batch, tokens, heads, head_dim):
 
 @pytest.mark.parametrize('plan', ['1,1,224', '1,1,96', '2,2,128', '1,1,64'])
 def test_linear_forced_tile_plans(ops, plan, monkeypatch):
-    """Tile plans the heuristic may not pick (BN not a multiple of the TMA-store box, clusters) stay correct."""
+    """Tile plans the heuristic may not pick (BN not a power of two, BN wider than the heuristic's, clusters with TMA
+    multicast) stay correct."""
     lib = _lib()
     monkeypatch.setenv('PE_GEMM_FORCE', plan)
     for epi_name in ('PE_EPI_F16', 'PE_EPI_F32'):
@@ -179,7 +181,7 @@ _TCGEN05_ATTENTION_CHECK = """
 import os, sys, torch
 import torch.nn.functional as F
 sys.path.insert(0, sys.argv[1])
-os.environ['PE_ATTN_TCGEN05'] = sys.argv[2]
+os.environ['PE_ATTN_WGMMA'] = sys.argv[2]
 from pipeedge_b200 import ops
 for batch, tokens, heads in [(2, 197, 12), (1, 128, 2), (3, 17, 2), (1, 64, 1), (1, 65, 1), (2, 198, 12), (1, 1, 1),
                              (1, 256, 2), (8, 197, 12), (4, 240, 3), (32, 128, 12), (16, 197, 16)]:
@@ -199,10 +201,10 @@ print('all ok')
 
 @pytest.mark.parametrize('mode', ['1', '0'])
 def test_attention_tcgen05(ops, mode):
-    """Both attention kernels - tcgen05 / TMEM (S and P in TMEM, V read MN-major from the TMA image; the default for
-    head_dim 64, S <= 256) and mma.sync (PE_ATTN_TCGEN05=0; also the fall-back for other shapes) - against fp32 maths over
-    S in {1 .. 256} incl. the ViT / DeiT / BERT shapes. The library reads its selector once per process, so each mode
-    runs in a child process."""
+    """Both attention kernels - wgmma (S in registers, P fed back from registers as the A operand, V read MN-major from
+    the TMA image; the default for head_dim 64, S <= 256) and mma.sync (PE_ATTN_WGMMA=0; also the fall-back for other
+    shapes) - against fp32 maths over S in {1 .. 256} incl. the ViT / DeiT / BERT shapes. The library reads its selector
+    once per process, so each mode runs in a child process."""
     import os
     import subprocess
     import sys
