@@ -8,6 +8,7 @@
 
 #include "../../include/pipeedge_b200.h"
 #include "common.cuh"
+#include "quant_dev.cuh"
 
 namespace pe {
 
@@ -73,15 +74,6 @@ int layernorm_impl(const void* x, const void* resid, const void* gamma, const vo
                    void* out_f32, void* out_f16, int rows, int hidden, cudaStream_t stream);
 int attention_impl(const void* qkv, void* ctx, int batch, int tokens, int heads, int head_dim, cudaStream_t stream);
 int cast_impl(const void* src, void* dst, size_t n, bool to_half, cudaStream_t stream);
-size_t quant_words(size_t n, int bit);
-size_t quant_workspace_bytes(int items, size_t n);
-int quant_encode_impl(const void* x, int items, size_t n, int bit, int clamp, void* codes, void* scale, void* shift,
-                      void* alpha, void* work, cudaStream_t stream);
-int quant_stats_impl(const void* x, int items, size_t n, int bit, int clamp, void* scale, void* shift, void* alpha,
-                     void* work, cudaStream_t stream);
-int quant_decode_impl(const void* codes, int items, size_t n, int bit, const void* scale, const void* shift, void* out,
-                      cudaStream_t stream);
-float clamp_factor(int bit, int gelu);
 void set_gemm_trace(void* buf);
 int gemm_plan_query(int m, int n, int k, int epilogue, int* out6);
 

@@ -38,11 +38,6 @@ namespace pe {
 
 void count_launches(int n);
 int require_sm90();
-float clamp_factor(int bit, int gelu);
-size_t quant_words(size_t n, int bit);
-size_t quant_workspace_bytes(int items, size_t n);
-int quant_encode_impl(const void* x, int items, size_t n, int bit, int clamp, void* codes, void* scale, void* shift,
-                      void* alpha, void* work, cudaStream_t stream);
 int add_impl(const void* a, const void* b, void* out, size_t n, cudaStream_t stream);
 
 constexpr int kPutThreads = 512;
@@ -154,15 +149,8 @@ __device__ void get_tensor(const uint8_t* slot, const LinkTensorHdr& th, int ti,
     return;
   }
   // QuantPipe decode (tensor_decode_outerdim, basic_op.py:146-176)
-  const int bit = static_cast<int>(th.bit);
-  const int ratio = 32 / bit;
-  const uint32_t mask = (1u << bit) - 1u;
-  const double levels = static_cast<double>(mask);
-  const bool use_lut = bit <= 12;
-  if (use_lut) {
-    for (uint32_t c = threadIdx.x; c <= mask; c += blockDim.x) lut[c] = dequant_unit(c, levels);
-    __syncthreads();
-  }
+  const QDecoder dec = fill_dequant_lut(lut, static_cast<int>(th.bit));
+  const int ratio = dec.ratio;
   const float* scale = reinterpret_cast<const float*>(slot + kLinkScaleOff + static_cast<size_t>(ti) * 4096);
   const float* shift = scale + kLinkMaxItems;
   const size_t wpi = (n + ratio - 1) / ratio;
@@ -192,10 +180,7 @@ __device__ void get_tensor(const uint8_t* slot, const LinkTensorHdr& th, int ti,
           for (int j = 0; j < ratio; j += 4) {
             float v[4];
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const uint32_t c = (ww[k] >> ((j + q) * bit)) & mask;
-              v[q] = dequant_value(use_lut ? lut[c] : dequant_unit(c, levels), sc, sh);
-            }
+            for (int q = 0; q < 4; ++q) v[q] = dec.value(ww[k], j + q, sc, sh);
             *reinterpret_cast<float4*>(oi + k * ratio + j) = make_float4(v[0], v[1], v[2], v[3]);
           }
         }
@@ -208,12 +193,7 @@ __device__ void get_tensor(const uint8_t* slot, const LinkTensorHdr& th, int ti,
     const size_t wi = w - item * wpi;
     const uint32_t word = __ldcg(codes + w);
     const float sc = __ldcg(scale + item), sh = __ldcg(shift + item);
-    float* oi = dst + item * n + wi * ratio;
-    for (int j = 0; j < ratio; ++j) {
-      if (wi * ratio + j >= n) break;
-      const uint32_t c = (word >> (j * bit)) & mask;
-      oi[j] = dequant_value(use_lut ? lut[c] : dequant_unit(c, levels), sc, sh);
-    }
+    dec.word(word, wi * ratio, n, sc, sh, dst + item * n + wi * ratio);
   }
 }
 
@@ -465,8 +445,7 @@ __global__ void __launch_bounds__(kPutThreads, 1) link_put_quant_kernel(const Pu
   extern __shared__ float4 cache4[];
   __shared__ uint64_t s_seq;
   __shared__ double red[kPutThreads / 32][kQPartialDoubles];
-  __shared__ double s_tot[kLinkMaxItems][3];
-  __shared__ float s_min[kLinkMaxItems], s_max[kLinkMaxItems];
+  __shared__ QStats s_item[kLinkMaxItems];
   __shared__ float s_alpha;
   constexpr int kWords = 16 * BIT / 32;
   constexpr int kRatio = 32 / BIT;
@@ -477,7 +456,6 @@ __global__ void __launch_bounds__(kPutThreads, 1) link_put_quant_kernel(const Pu
   const int segs = p.items * p.chunks;
   const size_t n = p.t.n;
   const uint32_t per4 = static_cast<uint32_t>(p.per >> 2);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   // ---------------------------------------------------------------- pass 1
   int local = 0;
@@ -485,8 +463,7 @@ __global__ void __launch_bounds__(kPutThreads, 1) link_put_quant_kernel(const Pu
     const int item = seg / p.chunks, chunk = seg - item * p.chunks;
     const size_t begin = static_cast<size_t>(chunk) * p.per;
     const size_t end = begin + p.per < n ? begin + p.per : n;
-    float mn = INFINITY, mx = -INFINITY;
-    double s = 0.0, ss = 0.0, ss32 = 0.0;
+    QStats st = QStats::empty();
     if (begin < end) {
       const uint32_t len4 = static_cast<uint32_t>((end - begin) >> 2);
       const float4* a4 = reinterpret_cast<const float4*>(p.t.a + static_cast<size_t>(item) * n + begin);
@@ -510,36 +487,11 @@ __global__ void __launch_bounds__(kPutThreads, 1) link_put_quant_kernel(const Pu
           float4 v = va[u];
           if (b4 != nullptr) { v.x += vb[u].x; v.y += vb[u].y; v.z += vb[u].z; v.w += vb[u].w; }
           if (p.cache) cache4[swz(off4 + i)] = v;
-          const float e[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            mn = fminf(mn, e[j]);
-            mx = fmaxf(mx, e[j]);
-            const double d = static_cast<double>(e[j]);
-            s += d;
-            ss += d * d;
-            ss32 += static_cast<double>(__fmul_rn(e[j], e[j]));
-          }
+          st.add(v);
         }
       }
     }
-    mn = warp_reduce(mn, [](float a, float b) { return fminf(a, b); });
-    mx = warp_max(mx);
-    s = warp_sum_d(s); ss = warp_sum_d(ss); ss32 = warp_sum_d(ss32);
-    __syncthreads();   // red[] of the previous segment has been read
-    if (lane == 0) {
-      red[warp][0] = mn; red[warp][1] = mx; red[warp][2] = s; red[warp][3] = ss; red[warp][4] = ss32;
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      double o0 = red[0][0], o1 = red[0][1], o2 = red[0][2], o3 = red[0][3], o4 = red[0][4];
-      for (int w = 1; w < kPutThreads / 32; ++w) {
-        o0 = fmin(o0, red[w][0]); o1 = fmax(o1, red[w][1]);
-        o2 += red[w][2]; o3 += red[w][3]; o4 += red[w][4];
-      }
-      double* q = p.tx.partials + static_cast<size_t>(seg) * kQPartialDoubles;
-      q[0] = o0; q[1] = o1; q[2] = o2; q[3] = o3; q[4] = o4;
-    }
+    stats_to_partial(st, red, p.tx.partials + static_cast<size_t>(seg) * kQPartialDoubles);
   }
   // ---------------------------------------------------------------- grid barrier
   __syncthreads();
@@ -561,34 +513,16 @@ __global__ void __launch_bounds__(kPutThreads, 1) link_put_quant_kernel(const Pu
   }
   __syncthreads();
   // ---------------------------------------------------------------- thresholds (same fixed order as quant_finalize_kernel)
-  for (int i = threadIdx.x; i < p.items; i += kPutThreads) {
-    double mn = INFINITY, mx = -INFINITY, s = 0.0, ss = 0.0, ss32 = 0.0;
-    for (int c = 0; c < p.chunks; ++c) {
-      const double* q = p.tx.partials + (static_cast<size_t>(i) * p.chunks + c) * kQPartialDoubles;
-      mn = fmin(mn, __ldcg(q)); mx = fmax(mx, __ldcg(q + 1));
-      s += __ldcg(q + 2); ss += __ldcg(q + 3); ss32 += __ldcg(q + 4);
-    }
-    s_min[i] = static_cast<float>(mn);
-    s_max[i] = static_cast<float>(mx);
-    s_tot[i][0] = s; s_tot[i][1] = ss; s_tot[i][2] = ss32;
-  }
+  for (int i = threadIdx.x; i < p.items; i += kPutThreads) s_item[i] = fold_item<true>(p.tx.partials, i, p.chunks);
   __syncthreads();
-  if (threadIdx.x == 0) {
-    double gmin = INFINITY, gs = 0.0, gss = 0.0, gss32 = 0.0;
-    for (int i = 0; i < p.items; ++i) {
-      gmin = fmin(gmin, static_cast<double>(s_min[i]));
-      gs += s_tot[i][0]; gss += s_tot[i][1]; gss32 += s_tot[i][2];
-    }
-    s_alpha = clamp_alpha(p.clamp, gmin, gs, gss, gss32, static_cast<double>(p.items) * static_cast<double>(n),
-                          p.factor_laplace, p.factor_gelu);
-  }
+  if (threadIdx.x == 0)
+    s_alpha = fold_items_alpha(p.items, [&](int i) { return s_item[i]; }, n, p.clamp, p.factor_laplace, p.factor_gelu);
   __syncthreads();
   const float alpha = s_alpha;
   if (blockIdx.x == 0 && threadIdx.x == 0) put_header(p, base, alpha);
   float* scale_out = reinterpret_cast<float*>(base + kLinkScaleOff + static_cast<size_t>(p.ti) * 4096);
   float* shift_out = scale_out + kLinkMaxItems;
   // ---------------------------------------------------------------- pass 2
-  const float levels = static_cast<float>((1u << BIT) - 1u);
   const size_t wpi = n / kRatio;   // n % 16 == 0
   uint32_t* codes = reinterpret_cast<uint32_t*>(base + p.data_off);
   local = 0;
@@ -596,10 +530,8 @@ __global__ void __launch_bounds__(kPutThreads, 1) link_put_quant_kernel(const Pu
     const int item = seg / p.chunks, chunk = seg - item * p.chunks;
     const size_t begin = static_cast<size_t>(chunk) * p.per;
     const size_t end = begin + p.per < n ? begin + p.per : n;
-    // clamp is monotonic: min / max of the clamped item = clamped min / max (basic_op.py:127-129)
-    const float sh = fminf(fmaxf(s_min[item], -alpha), alpha);
-    const float hi = fminf(fmaxf(s_max[item], -alpha), alpha);
-    const float sc = __fsub_rn(hi, sh);
+    float sc, sh;
+    item_scale_shift(s_item[item].mn, s_item[item].mx, alpha, sc, sh);
     if (chunk == 0 && threadIdx.x == 0) {
       scale_out[item] = sc;
       shift_out[item] = sh;
@@ -624,29 +556,7 @@ __global__ void __launch_bounds__(kPutThreads, 1) link_put_quant_kernel(const Pu
           }
         }
       }
-      uint32_t q[16];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        q[4 * j + 0] = quant_code(v[j].x, alpha, sh, sc, levels);
-        q[4 * j + 1] = quant_code(v[j].y, alpha, sh, sc, levels);
-        q[4 * j + 2] = quant_code(v[j].z, alpha, sh, sc, levels);
-        q[4 * j + 3] = quant_code(v[j].w, alpha, sh, sc, levels);
-      }
-      uint32_t w[kWords];
-#pragma unroll
-      for (int k = 0; k < kWords; ++k) {
-        uint32_t acc = 0;
-#pragma unroll
-        for (int j = 0; j < kRatio; ++j) acc |= q[k * kRatio + j] << (j * BIT);
-        w[k] = acc;
-      }
-      uint32_t* dst = ci + static_cast<size_t>(u) * kWords;
-      if (kWords == 1) dst[0] = w[0];
-      else if (kWords == 2) *reinterpret_cast<uint2*>(dst) = make_uint2(w[0], w[1]);
-      else {
-#pragma unroll
-        for (int k = 0; k < kWords; k += 4) *reinterpret_cast<uint4*>(dst + k) = make_uint4(w[k], w[k + 1], w[k + 2], w[k + 3]);
-      }
+      pack16<BIT>(v, alpha, sh, sc).store(ci + static_cast<size_t>(u) * kWords);
     }
   }
   put_end(p, seq);
@@ -840,7 +750,7 @@ int link_put(pe_link* l, const PutTensor* t, int n_tensors, int items, int bit, 
       link_put_copy_kernel<<<grid, kPutThreads, 0, stream>>>(p);
       PE_CUDA(cudaGetLastError());
       count_launches(1);
-    } else if ((bit == 2 || bit == 4 || bit == 8 || bit == 16) && t[ti].n % 16 == 0 && aligned) {
+    } else if (quant_pack16_applies(bit, t[ti].n, aligned)) {
       // segments: `chunks` per item so that items * chunks ~ the grid; boundaries on multiples of 16 elements
       const int grid_cap = sm_count() > 16 ? sm_count() - 8 : sm_count();
       int chunks = items >= grid_cap ? 1 : grid_cap / items;

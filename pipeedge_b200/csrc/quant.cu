@@ -45,59 +45,15 @@ quant_stats_kernel(const float* __restrict__ x, size_t n, int chunks, double* __
   const size_t per = ((n + chunks - 1) / chunks + 3) & ~static_cast<size_t>(3);
   const size_t begin = static_cast<size_t>(chunk) * per;
   const size_t end = begin + per < n ? begin + per : n;
-  float mn = INFINITY, mx = -INFINITY;
-  double s = 0.0, ss = 0.0, ss32 = 0.0;
+  // float4 body when xi is 16-byte aligned, then the scalar rest
   const bool vec = ((reinterpret_cast<uintptr_t>(xi) & 15) == 0);
-  if (begin < end) {
-    if (vec) {
-      const size_t nv = (end - begin) >> 2;
-      const float4* x4 = reinterpret_cast<const float4*>(xi + begin);
-      for (size_t i = threadIdx.x; i < nv; i += kQStatThreads) {
-        const float4 v = x4[i];
-        const float e[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          mn = fminf(mn, e[j]);
-          mx = fmaxf(mx, e[j]);
-          const double d = static_cast<double>(e[j]);
-          s += d;
-          ss += d * d;
-          ss32 += static_cast<double>(__fmul_rn(e[j], e[j]));
-        }
-      }
-      for (size_t i = begin + (nv << 2) + threadIdx.x; i < end; i += kQStatThreads) {
-        const float e = xi[i];
-        mn = fminf(mn, e); mx = fmaxf(mx, e);
-        const double d = static_cast<double>(e);
-        s += d; ss += d * d; ss32 += static_cast<double>(__fmul_rn(e, e));
-      }
-    } else {
-      for (size_t i = begin + threadIdx.x; i < end; i += kQStatThreads) {
-        const float e = xi[i];
-        mn = fminf(mn, e); mx = fmaxf(mx, e);
-        const double d = static_cast<double>(e);
-        s += d; ss += d * d; ss32 += static_cast<double>(__fmul_rn(e, e));
-      }
-    }
-  }
-  mn = warp_reduce(mn, [](float a, float b) { return fminf(a, b); });
-  mx = warp_max(mx);
-  s = warp_sum_d(s); ss = warp_sum_d(ss); ss32 = warp_sum_d(ss32);
+  const size_t nv = vec && begin < end ? (end - begin) >> 2 : 0;
+  const float4* x4 = reinterpret_cast<const float4*>(xi + begin);
+  QStats st = QStats::empty();
+  for (size_t i = threadIdx.x; i < nv; i += kQStatThreads) st.add(x4[i]);
+  for (size_t i = begin + (nv << 2) + threadIdx.x; i < end; i += kQStatThreads) st.add(xi[i]);
   __shared__ double red[kQStatThreads / 32][kQPartialDoubles];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (lane == 0) {
-    red[warp][0] = mn; red[warp][1] = mx; red[warp][2] = s; red[warp][3] = ss; red[warp][4] = ss32;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double o0 = red[0][0], o1 = red[0][1], o2 = red[0][2], o3 = red[0][3], o4 = red[0][4];
-    for (int w = 1; w < kQStatThreads / 32; ++w) {
-      o0 = fmin(o0, red[w][0]); o1 = fmax(o1, red[w][1]);
-      o2 += red[w][2]; o3 += red[w][3]; o4 += red[w][4];
-    }
-    double* p = partials + (static_cast<size_t>(item) * chunks + chunk) * kQPartialDoubles;
-    p[0] = o0; p[1] = o1; p[2] = o2; p[3] = o3; p[4] = o4;
-  }
+  stats_to_partial(st, red, partials + (static_cast<size_t>(item) * chunks + chunk) * kQPartialDoubles);
 }
 
 // ------------------------------------------------------------------ pass 1b: thresholds (one block)
@@ -113,41 +69,25 @@ __global__ void quant_finalize_kernel(double* partials, int items, int chunks, s
   // thread 0 over the items (the per-item sums are parked in the partials' first chunk slot)
   __shared__ float s_alpha;
   for (int i = threadIdx.x; i < items; i += blockDim.x) {
-    double mn = INFINITY, mx = -INFINITY, s = 0.0, ss = 0.0, ss32 = 0.0;
-    for (int c = 0; c < chunks; ++c) {
-      const double* p = partials + (static_cast<size_t>(i) * chunks + c) * kQPartialDoubles;
-      mn = fmin(mn, p[0]); mx = fmax(mx, p[1]);
-      s += p[2]; ss += p[3]; ss32 += p[4];
-    }
-    item_min[i] = static_cast<float>(mn);
-    item_max[i] = static_cast<float>(mx);
+    const QStats t = fold_item<false>(partials, i, chunks);
+    item_min[i] = t.mn;
+    item_max[i] = t.mx;
     double* p0 = partials + static_cast<size_t>(i) * chunks * kQPartialDoubles;
-    p0[0] = mn; p0[2] = s; p0[3] = ss; p0[4] = ss32;
+    p0[2] = t.s; p0[3] = t.ss; p0[4] = t.ss32;
   }
   __syncthreads();
   if (threadIdx.x == 0) {
-    double gmin = INFINITY, gs = 0.0, gss = 0.0, gss32 = 0.0;
-    for (int i = 0; i < items; ++i) {
+    const float alpha = fold_items_alpha(items, [&](int i) {
       const double* p0 = partials + static_cast<size_t>(i) * chunks * kQPartialDoubles;
-      gmin = fmin(gmin, p0[0]);
-      gs += p0[2]; gss += p0[3]; gss32 += p0[4];
-    }
-    // clamp_op.py:11-33 (see clamp_alpha in quant_dev.cuh; the fused send kernel of link.cu shares it)
-    const float alpha = clamp_alpha(clamp, gmin, gs, gss, gss32, static_cast<double>(items) * static_cast<double>(n),
-                                    factor_laplace, factor_gelu);
+      return QStats{item_min[i], item_max[i], p0[2], p0[3], p0[4]};
+    }, n, clamp, factor_laplace, factor_gelu);
     s_alpha = alpha;
     hdr->alpha = alpha;
     if (alpha_out != nullptr) *alpha_out = alpha;
   }
   __syncthreads();
   const float alpha = s_alpha;
-  for (int i = threadIdx.x; i < items; i += blockDim.x) {
-    // clamp is monotonic: min/max of the clamped item = clamped min/max (basic_op.py:127-129)
-    const float lo = fminf(fmaxf(item_min[i], -alpha), alpha);
-    const float hi = fminf(fmaxf(item_max[i], -alpha), alpha);
-    shift[i] = lo;
-    scale[i] = __fsub_rn(hi, lo);
-  }
+  for (int i = threadIdx.x; i < items; i += blockDim.x) item_scale_shift(item_min[i], item_max[i], alpha, scale[i], shift[i]);
 }
 
 // ------------------------------------------------------------------ pass 2: quantise + pack
@@ -163,7 +103,6 @@ quant_pack16_kernel(const float* __restrict__ x, size_t n, const QuantHeader* __
   const size_t groups = n >> 4;
   const float alpha = hdr->alpha;
   const float sh = shift[item], sc = scale[item];
-  const float levels = static_cast<float>((1u << BIT) - 1u);
   const float4* xi = reinterpret_cast<const float4*>(x + static_cast<size_t>(item) * n);
   uint32_t* ci = codes + static_cast<size_t>(item) * words_per_item;
   for (size_t g = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; g < groups;
@@ -171,30 +110,7 @@ quant_pack16_kernel(const float* __restrict__ x, size_t n, const QuantHeader* __
     float4 v[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) v[j] = xi[g * 4 + j];
-    uint32_t q[16];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      q[4 * j + 0] = quant_code(v[j].x, alpha, sh, sc, levels);
-      q[4 * j + 1] = quant_code(v[j].y, alpha, sh, sc, levels);
-      q[4 * j + 2] = quant_code(v[j].z, alpha, sh, sc, levels);
-      q[4 * j + 3] = quant_code(v[j].w, alpha, sh, sc, levels);
-    }
-    uint32_t w[kWords];
-    constexpr int kRatio = 32 / BIT;
-#pragma unroll
-    for (int k = 0; k < kWords; ++k) {
-      uint32_t acc = 0;
-#pragma unroll
-      for (int j = 0; j < kRatio; ++j) acc |= q[k * kRatio + j] << (j * BIT);
-      w[k] = acc;
-    }
-    uint32_t* dst = ci + g * kWords;
-    if (kWords == 1) dst[0] = w[0];
-    else if (kWords == 2) *reinterpret_cast<uint2*>(dst) = make_uint2(w[0], w[1]);
-    else {
-#pragma unroll
-      for (int k = 0; k < kWords; k += 4) *reinterpret_cast<uint4*>(dst + k) = make_uint4(w[k], w[k + 1], w[k + 2], w[k + 3]);
-    }
+    pack16<BIT>(v, alpha, sh, sc).store(ci + g * kWords);
   }
 }
 
@@ -226,32 +142,16 @@ quant_pack_generic_kernel(const float* __restrict__ x, size_t n, int bit, const 
 __global__ void __launch_bounds__(256)
 quant_decode_kernel(const uint32_t* __restrict__ codes, size_t n, int bit, size_t words_per_item,
                     const float* __restrict__ scale, const float* __restrict__ shift, float* __restrict__ out) {
-  // _intmap2float: float32(code / (2^bit - 1)) with a float64 divide. A shared-memory table of the
-  // 2^bit possible values replaces the divide for bit <= 12.
   extern __shared__ float lut[];
   const int item = blockIdx.y;
-  const int ratio = 32 / bit;
-  const uint32_t mask = (1u << bit) - 1u;
-  const double levels = static_cast<double>(mask);
-  const bool use_lut = bit <= 12;
-  if (use_lut) {
-    for (uint32_t c = threadIdx.x; c <= mask; c += blockDim.x) lut[c] = dequant_unit(c, levels);
-    __syncthreads();
-  }
+  const QDecoder dec = fill_dequant_lut(lut, bit);
   const float sc = scale[item], sh = shift[item];
   const uint32_t* ci = codes + static_cast<size_t>(item) * words_per_item;
   float* oi = out + static_cast<size_t>(item) * n;
   for (size_t w = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; w < words_per_item;
        w += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const uint32_t word = ci[w];
-    const size_t e0 = w * ratio;
-    for (int j = 0; j < ratio; ++j) {
-      const size_t e = e0 + j;
-      if (e >= n) break;
-      const uint32_t c = (word >> (j * bit)) & mask;
-      const float v = use_lut ? lut[c] : dequant_unit(c, levels);
-      oi[e] = dequant_value(v, sc, sh);  // basic_op.py:163: two fp32 roundings
-    }
+    const size_t e0 = w * dec.ratio;
+    dec.word(ci[w], e0, n, sc, sh, oi + e0);
   }
 }
 
@@ -315,9 +215,7 @@ int quant_encode_impl(const void* x, int items, size_t n, int bit, int clamp, vo
   const float* xf = static_cast<const float*>(x);
   const size_t words = quant_words(n, bit);
   uint32_t* cw = static_cast<uint32_t*>(codes);
-  const bool fast = (n % 16 == 0) && ((reinterpret_cast<uintptr_t>(x) & 15) == 0) &&
-                    (bit == 2 || bit == 4 || bit == 8 || bit == 16);
-  if (fast) {
+  if (quant_pack16_applies(bit, n, (reinterpret_cast<uintptr_t>(x) & 15) == 0)) {
     const size_t groups = n / 16;
     size_t bx = (groups + 255) / 256;
     const size_t cap = static_cast<size_t>(kNumSMs) * 8 / static_cast<size_t>(items) + 1;
