@@ -10,15 +10,16 @@ for one rank per GPU:
 * The DEVICE of a tensor picks its plane. CUDA tensors (activations, int8 codes, per-item scales) travel
   over a dedicated 2-rank NCCL communicator per hop direction on a side stream, ordered against the compute
   stream with CUDA events, so the hop of micro-batch i overlaps the compute of micro-batch i+1 without the
-  host ever waiting on the GPU. CPU tensors and the (cached) payload header travel over Gloo, as every
-  message does in the reference (`p2p/__init__.py:96-121`).
+  host ever waiting on the GPU. CPU tensors and the (cached) payload header travel over the hop's socket,
+  where the reference sends every message over Gloo (`p2p/__init__.py:96-121`).
 * One NCCL communicator per ordered rank pair: the reference's send and receive threads run concurrently
   (`p2p/__init__.py:155-258`) and NCCL serialises a communicator's operations on one internal stream, so a
   shared communicator could deadlock when two ranks send to each other (stage 0 <-> last stage on 2 ranks).
 * The command channel (`cmd_broadcast`, `CommandThread`; `p2p/__init__.py:75-85,298-331`) stays on Gloo:
   NCCL has neither tags nor any-source receive.
 
-Without CUDA (the CPU test-suite) everything rides Gloo and the classes behave like the reference's.
+Without CUDA (the CPU test-suite) payloads ride the hop sockets alone and the classes behave like the reference's.
+With CUDA, a process that cannot load libnccl.so.2 refuses to open a hop; there is no second data plane.
 """
 import collections
 import logging
@@ -66,11 +67,14 @@ def ring_slots() -> int:
 
 
 def _native_lib():
-    """`libpipeedge_b200.so` when this process drives a GPU (native hop fast path), else None."""
+    """`libpipeedge_b200.so` when this process drives a GPU (its hops carry CUDA payloads over NCCL), else None."""
     if not torch.cuda.is_available():
         return None
     from ..._lib import LIB   # pylint: disable=import-outside-toplevel
-    return LIB if LIB.pe_hop_available() else None
+    if not LIB.pe_hop_available():
+        raise RuntimeError("libnccl.so.2 cannot be loaded in this process; the hops' CUDA payloads travel over NCCL "
+                           "(a CUDA build of PyTorch ships and loads it)")
+    return LIB
 
 
 _NCCL_HOPS_OPENED = 0
@@ -162,15 +166,14 @@ class DistP2pContext(DistContext):
     """The singleton distributed P2P context manager (`p2p/__init__.py:41-85`).
 
     Parameters are the reference's: `ipg_args` / `ipg_kwargs` for `torch.distributed.init_process_group()`
-    (the default group is the Gloo control plane) and the command handler `cmd_cb`. When CUDA is available, one
-    NCCL process group per ordered rank pair is created for the data plane.
+    (the default group is the Gloo control plane) and the command handler `cmd_cb`. The data plane is not a process
+    group: each hop's exchange threads open its socket and, with CUDA, its NCCL communicator (`_NativeHop`).
     """
     _instance: Optional['DistP2pContext'] = None
 
     def __init__(self, ipg_args: tuple, ipg_kwargs: dict, cmd_cb: DistCmdHandler):
         super().__init__(ipg_args, ipg_kwargs)
         self._thread_cmd = CommandThread(cmd_cb)
-        self._hop_groups = {}
         self._listener = None
         self._sock_path = None
         self._inbound = {}                      # src rank -> accepted connection
@@ -180,12 +183,6 @@ class DistP2pContext(DistContext):
         """Initialize the distributed context and threads."""
         super().init()
         dist.init_process_group(*self._init_args, **self._init_kwargs)
-        if torch.cuda.is_available() and self._world_size > 1 and _native_lib() is None:
-            # fallback data plane (torch.distributed NCCL): every rank must create every group, in the same order
-            for src in range(self._world_size):
-                for dst in range(self._world_size):
-                    if src != dst:
-                        self._hop_groups[(src, dst)] = dist.new_group(ranks=[src, dst], backend='nccl')
         if self._world_size > 1:
             self._sock_path = self.sock_path(self._rank)
             if os.path.exists(self._sock_path):
@@ -261,12 +258,6 @@ class DistP2pContext(DistContext):
                 if time.monotonic() > deadline:
                     raise
                 time.sleep(0.01)
-
-    @classmethod
-    def hop_group(cls, src: int, dst: int):
-        """NCCL group for the directed hop `src -> dst` (None when the data plane is Gloo)."""
-        inst = cls._instance
-        return None if inst is None else inst._hop_groups.get((src, dst))   # pylint: disable=protected-access
 
     def cmd_broadcast(self, cmd: int, tensors: Optional[Tuple[torch.Tensor, ...]] = None) -> None:
         """Broadcast a command with optional (CPU) tensors to every other rank (`p2p/__init__.py:72-85`)."""
@@ -427,11 +418,10 @@ class TensorSendThread(AbstractTensorExchangeThread):
     def run(self):
         """Dequeue payloads and send them."""
         self._enter_device()
-        group = DistP2pContext.hop_group(dist.get_rank(), self._dst_rank)
         if self._sock is None:
             self.open_hop()
         try:
-            self._run(group)
+            self._run()
         finally:
             if self._hop is not None and self._inflight:
                 self._inflight[-1].synchronize()     # every send has left: the peer's matching receives complete too
@@ -478,7 +468,7 @@ class TensorSendThread(AbstractTensorExchangeThread):
         self._sock.sendall(b''.join([_ENV_HEAD.pack(len(meta), blob_len), meta, *parts]))
         return False
 
-    def _run(self, group):
+    def _run(self):
         while not self._evt_stop_thread.is_set():
             t_wait = time.perf_counter()
             with self._queue_out.condition:
@@ -496,11 +486,12 @@ class TensorSendThread(AbstractTensorExchangeThread):
             tensors = [o for o in objs if isinstance(o, torch.Tensor)]
             cpu = [t for t in tensors if not t.is_cuda]
             cuda = [t for t in tensors if t.is_cuda]
-            hop = self._hop if cuda else None
-            fast = self._send_envelope(_signature(objs, is_tuple), cpu, defer_fast=hop is not None)
+            fast = self._send_envelope(_signature(objs, is_tuple), cpu, defer_fast=bool(cuda))
             self._call_pre_hooks()
-            if hop is not None:
-                # native fast path: envelope header + NCCL sends + event record in one GIL-free call
+            if cuda:
+                # envelope header + NCCL sends + event record in one GIL-free call (CUDA tensors exist only in a process
+                # with CUDA, where open_hop has joined the hop's communicator)
+                hop = self._hop
                 for tensor in cuda:
                     tensor.record_stream(self._stream)
                 if self._timing_hooks:
@@ -520,28 +511,7 @@ class TensorSendThread(AbstractTensorExchangeThread):
                 if payload.on_consumed is not None:
                     payload.on_consumed(done)
                 self._inflight.append(done)
-                while len(self._inflight) > 1 + queue_depth():
-                    self._inflight.popleft().synchronize()
-            elif cuda:
-                if group is None:
-                    raise RuntimeError("CUDA tensors in a payload need the NCCL data plane (DistP2pContext with CUDA)")
-                with torch.cuda.stream(self._stream):
-                    if payload.ready is not None:
-                        self._stream.wait_event(payload.ready)
-                    for tensor in cuda:
-                        tensor.record_stream(self._stream)
-                    if len(cuda) == 1:
-                        dist.isend(cuda[0], self._dst_rank, group=group).wait()   # stream-level wait: host does not block
-                    else:
-                        ops = [dist.P2POp(dist.isend, t, self._dst_rank, group=group) for t in cuda]
-                        for work in dist.batch_isend_irecv(ops):   # one ncclGroup for the whole payload
-                            work.wait()
-                    done = torch.cuda.Event()
-                    done.record(self._stream)
-                if payload.on_consumed is not None:
-                    payload.on_consumed(done)
                 # bound the number of sends the host may run ahead of the device
-                self._inflight.append(done)
                 while len(self._inflight) > 1 + queue_depth():
                     self._inflight.popleft().synchronize()
             elif payload.on_consumed is not None:
@@ -583,12 +553,11 @@ class TensorRecvThread(AbstractTensorExchangeThread):
     def run(self):
         """Receive payloads and enqueue them."""
         self._enter_device()
-        group = DistP2pContext.hop_group(self._src_rank, dist.get_rank())
         if self._conn is None:
             self.open_hop()
         conn, hop = self._conn, self._hop
         try:
-            self._loop(conn, hop, group)
+            self._loop(conn, hop)
         finally:
             if hop is not None:
                 if self._stream is not None:
@@ -602,7 +571,7 @@ class TensorRecvThread(AbstractTensorExchangeThread):
         lib = _native_lib()
         self._hop = _NativeHop(lib, self._conn, False) if lib is not None else None
 
-    def _loop(self, conn, hop, group):
+    def _loop(self, conn, hop):
         while True:
             # blocks until the sender's next payload or its closing envelope (sent by its shutdown); no polling
             # thread per message as in the reference (`p2p/__init__.py:224-232`)
@@ -657,26 +626,9 @@ class TensorRecvThread(AbstractTensorExchangeThread):
                 self._last_cpu = new_cpu
             ready = None
             on_consumed = None
-            if cuda_slots and hop is not None:
+            if cuda_slots:   # device buffers exist only with CUDA, where open_hop has joined the hop's communicator
                 ready = _fresh_event(self._stream)
                 hop.recv(cuda_slots, self._stream, ready)
-
-                def on_consumed(evt, slots=tuple(cuda_slots)):
-                    for slot in slots:
-                        slot[1] = evt
-            elif cuda_slots:
-                with torch.cuda.stream(self._stream):
-                    for slot in cuda_slots:
-                        if slot[1] is not None:
-                            self._stream.wait_event(slot[1])    # the previous consumer of this buffer is done
-                    if len(cuda_slots) == 1:
-                        dist.irecv(cuda_slots[0][0], self._src_rank, group=group).wait()
-                    else:
-                        ops = [dist.P2POp(dist.irecv, slot[0], self._src_rank, group=group) for slot in cuda_slots]
-                        for work in dist.batch_isend_irecv(ops):
-                            work.wait()
-                    ready = torch.cuda.Event()
-                    ready.record(self._stream)
 
                 def on_consumed(evt, slots=tuple(cuda_slots)):
                     for slot in slots:

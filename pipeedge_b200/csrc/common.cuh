@@ -25,6 +25,11 @@ int check_cuda(cudaError_t err, const char* what);
     }                                                  \
   } while (0)
 
+// ---------------------------------------------------------------- stream sockets (hop.cu)
+// Send / receive all n bytes, retrying on EINTR: 0 ok, -1 error (errno says why); read_all returns 1 at EOF.
+int write_all(int fd, const void* buf, size_t n);
+int read_all(int fd, void* buf, size_t n);
+
 constexpr int kNumSMs = 132;  // H100 SXM
 
 // ---------------------------------------------------------------- small utilities

@@ -75,7 +75,7 @@ static std::mutex& comm_lifecycle_mutex() {
   return m;
 }
 
-static int write_all(int fd, const void* buf, size_t n) {
+int write_all(int fd, const void* buf, size_t n) {
   const char* p = static_cast<const char*>(buf);
   while (n > 0) {
     const ssize_t w = send(fd, p, n, MSG_NOSIGNAL);
@@ -89,7 +89,7 @@ static int write_all(int fd, const void* buf, size_t n) {
   return 0;
 }
 
-static int read_all(int fd, void* buf, size_t n) {
+int read_all(int fd, void* buf, size_t n) {
   char* p = static_cast<char*>(buf);
   while (n > 0) {
     const ssize_t r = recv(fd, p, n, 0);

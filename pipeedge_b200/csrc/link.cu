@@ -64,32 +64,27 @@ __device__ __forceinline__ unsigned ld_acquire_gpu_u32(const unsigned* p) {
   asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
   return v;
 }
-__device__ __forceinline__ uint64_t ld_flag(const uint64_t* p, int relaxed) {
-  // relaxed: a volatile load (never served from L1); payload reads that follow use ld.global.cg, i.e. L2 - the point of
-  // coherence peer and DMA writes land in - so no acquire fence is needed to see the data the flag announces
-  return relaxed ? *reinterpret_cast<const volatile uint64_t*>(p) : ld_acquire_sys(p);
-}
-// Bounded: a protocol bug or a dead peer ends in a trap (the launch fails, the host sees an error), never in a hang.
-__device__ __forceinline__ void spin_until_ge(const uint64_t* flag, uint64_t want, unsigned long long timeout_ns,
-                                              unsigned* status, unsigned code, int relaxed = 0) {
-  if (ld_flag(flag, relaxed) >= want) return;
-  const unsigned long long t0 = globaltimer_ns();
-  unsigned ns = 32;
-  while (ld_flag(flag, relaxed) < want) {
-    __nanosleep(ns);
-    if (ns < 512) ns <<= 1;
-    if (globaltimer_ns() - t0 > timeout_ns) {
-      *reinterpret_cast<volatile unsigned*>(status) = code;
-      __threadfence_system();
-      printf("pipeedge_b200: link wait timed out (code %u, block %d)\n", code, blockIdx.x);
-      __trap();
-    }
-  }
-}
 __device__ __forceinline__ void fail(unsigned* status, unsigned code) {
   *reinterpret_cast<volatile unsigned*>(status) = code;
   __threadfence_system();
   __trap();
+}
+// Bounded: a protocol bug or a dead peer ends in a trap (the launch fails, the host sees an error), never in a hang.
+// Between polls the back-off doubles from kMinNs up to kMaxNs.
+template <unsigned kMinNs, unsigned kMaxNs>
+__device__ __forceinline__ void spin_until_ge(const uint64_t* flag, uint64_t want, unsigned long long timeout_ns,
+                                              unsigned* status, unsigned code) {
+  if (ld_acquire_sys(flag) >= want) return;
+  const unsigned long long t0 = globaltimer_ns();
+  unsigned ns = kMinNs;
+  while (ld_acquire_sys(flag) < want) {
+    __nanosleep(ns);
+    if (ns < kMaxNs) ns <<= 1;
+    if (globaltimer_ns() - t0 > timeout_ns) {
+      printf("pipeedge_b200: link wait timed out (code %u, block %d)\n", code, blockIdx.x);
+      fail(status, code);
+    }
+  }
 }
 
 // ------------------------------------------------------------------------------------------------ get
@@ -101,7 +96,6 @@ struct GetArgs {
   int items;
   int n_tensors;
   int raw;              // host-fed link: no header, copy n0 bytes
-  int sync_mode;
   unsigned long long timeout_ns;
 };
 
@@ -204,20 +198,7 @@ __global__ void __launch_bounds__(32) link_wait_kernel(const LinkRx rx, unsigned
   if (threadIdx.x == 0) {
     const uint64_t seq = *reinterpret_cast<volatile uint64_t*>(rx.seq);
     const uint64_t slot = seq % static_cast<uint64_t>(rx.n_slots), k = seq / static_cast<uint64_t>(rx.n_slots);
-    const uint64_t* flag = rx.full + slot;
-    if (ld_acquire_sys(flag) >= k + 1) return;
-    const unsigned long long t0 = globaltimer_ns();
-    unsigned ns = 64;
-    while (ld_acquire_sys(flag) < k + 1) {
-      __nanosleep(ns);
-      if (ns < 2048) ns <<= 1;
-      if (globaltimer_ns() - t0 > timeout_ns) {
-        *reinterpret_cast<volatile unsigned*>(rx.status) = kLinkErrWaitFull;
-        __threadfence_system();
-        printf("pipeedge_b200: link wait timed out (consumer, slot %llu)\n", static_cast<unsigned long long>(slot));
-        __trap();
-      }
-    }
+    spin_until_ge<64, 2048>(rx.full + slot, k + 1, timeout_ns, rx.status, kLinkErrWaitFull);
   }
 }
 
@@ -227,7 +208,7 @@ __global__ void __launch_bounds__(kGetThreads) link_get_kernel(const GetArgs g) 
   if (threadIdx.x == 0) {
     const uint64_t seq = *reinterpret_cast<volatile uint64_t*>(g.rx.seq);
     const uint64_t slot = seq % static_cast<uint64_t>(g.rx.n_slots), k = seq / static_cast<uint64_t>(g.rx.n_slots);
-    spin_until_ge(g.rx.full + slot, k + 1, g.timeout_ns, g.rx.status, kLinkErrWaitFull, g.sync_mode & 1);
+    spin_until_ge<32, 512>(g.rx.full + slot, k + 1, g.timeout_ns, g.rx.status, kLinkErrWaitFull);
     s_seq = seq;
   }
   __syncthreads();
@@ -269,12 +250,14 @@ __global__ void __launch_bounds__(kGetThreads) link_get_kernel(const GetArgs g) 
       get_tensor(base, h.t[1], 1, g.items, static_cast<float*>(g.dst1), get_lut);
     }
   }
-  // every CTA has finished reading -> hand the slot back to the producer. One fence per CTA, after its barrier (the
-  // fence is cumulative over what the barrier ordered before it): a system-scope fence in every thread made these
-  // kernels 3-4x longer than their copy (ncu r02c).
+  // every CTA has finished reading -> hand the slot back to the producer. One GPU-scope fence per CTA, after its barrier
+  // (the fence is cumulative over what the barrier ordered before it); the CTA that arrives last releases the slot with
+  // a system-scope fence and st.release.sys, which are cumulative over everything the arrival counter ordered before
+  // them. A system-scope fence in every thread made these kernels 3-4x longer than their copy (ncu r02c), and one in
+  // every CTA makes each CTA wait for its own accesses to become visible system-wide.
   __syncthreads();
   if (threadIdx.x == 0) {
-    if (g.sync_mode & 2) __threadfence(); else __threadfence_system();
+    __threadfence();
     const unsigned prev = atomicAdd(g.rx.done_ctr, 1u);
     if (prev == gridDim.x - 1) {
       *g.rx.done_ctr = 0;
@@ -298,7 +281,6 @@ struct PutArgs {
   int chunks;             // fused quantise: segments per item
   size_t per;             // ... elements per segment (multiple of 16)
   int cache;              // ... keep the fp32 slice in shared memory between the passes
-  int sync_mode;
   unsigned long long timeout_ns;
   // staged path (generic bit-widths): codes / scale / shift already computed into local memory
   const uint8_t* staged_codes;
@@ -312,7 +294,7 @@ __device__ __forceinline__ void put_begin(const PutArgs& p, uint64_t* s_seq) {
   if (threadIdx.x == 0) {
     const uint64_t seq = *reinterpret_cast<volatile uint64_t*>(p.tx.seq);
     const uint64_t slot = seq % static_cast<uint64_t>(p.tx.n_slots), k = seq / static_cast<uint64_t>(p.tx.n_slots);
-    spin_until_ge(p.tx.free_ + slot, k, p.timeout_ns, p.tx.status, kLinkErrWaitFree, p.sync_mode & 1);   // (k-1)-th use consumed
+    spin_until_ge<32, 512>(p.tx.free_ + slot, k, p.timeout_ns, p.tx.status, kLinkErrWaitFree);   // (k-1)-th use consumed
     *s_seq = seq;
   }
   __syncthreads();
@@ -337,11 +319,12 @@ __device__ __forceinline__ void put_header(const PutArgs& p, uint8_t* base, floa
 }
 
 __device__ __forceinline__ void put_end(const PutArgs& p, uint64_t seq) {
-  // this CTA's peer stores are ordered before its arrival (barrier, then ONE cumulative system-scope fence); the last
-  // CTA to arrive publishes the slot
+  // this CTA's peer stores are ordered before its arrival (barrier, then ONE GPU-scope fence); the last CTA to arrive
+  // publishes the slot with a system-scope fence and st.release.sys, cumulative over what the arrival counter ordered
+  // before them (see the end of link_get_kernel)
   __syncthreads();
   if (threadIdx.x == 0) {
-    if (p.sync_mode & 2) __threadfence(); else __threadfence_system();
+    __threadfence();
     const unsigned prev = atomicAdd(p.tx.done_ctr, 1u);
     if (prev == gridDim.x - 1) {
       *p.tx.done_ctr = 0;
@@ -563,34 +546,6 @@ __global__ void __launch_bounds__(kPutThreads, 1) link_put_quant_kernel(const Pu
 }
 
 // ------------------------------------------------------------------------------------------------ host helpers
-static int write_all(int fd, const void* buf, size_t n) {
-  const char* p = static_cast<const char*>(buf);
-  while (n > 0) {
-    const ssize_t w = send(fd, p, n, MSG_NOSIGNAL);
-    if (w < 0) {
-      if (errno == EINTR) continue;
-      return -1;
-    }
-    p += w;
-    n -= static_cast<size_t>(w);
-  }
-  return 0;
-}
-static int read_all(int fd, void* buf, size_t n) {
-  char* p = static_cast<char*>(buf);
-  while (n > 0) {
-    const ssize_t r = recv(fd, p, n, 0);
-    if (r == 0) return 1;   // EOF
-    if (r < 0) {
-      if (errno == EINTR) continue;
-      return -1;
-    }
-    p += r;
-    n -= static_cast<size_t>(r);
-  }
-  return 0;
-}
-
 static unsigned long long default_timeout_ns() {
   const char* e = getenv("PIPEEDGE_LINK_TIMEOUT_S");
   double s = e != nullptr ? atof(e) : 30.0;
@@ -633,13 +588,6 @@ static int alloc_common(pe_link* l) {
   preload_kernels();
   const char* w = getenv("PIPEEDGE_WIRE_F16");
   l->wire_f16 = (w != nullptr && w[0] == '1') ? 1 : 0;
-  // Default 2: one GPU-scope fence per CTA, one system-scope fence by the CTA that publishes the slot (the release is
-  // cumulative over what the arrival counter ordered before it): a system-scope fence in every CTA makes each CTA wait
-  // for its stores to become visible system-wide. PE_LINK_SYNC=0 restores that stricter mode.
-  const char* sm = getenv("PE_LINK_SYNC");
-  l->sync_mode = sm != nullptr ? atoi(sm) : 2;
-  const char* gc = getenv("PE_LINK_GRID_CAP");
-  l->grid_cap = gc != nullptr ? atoi(gc) : 0;
   return PE_OK;
 }
 
@@ -736,7 +684,6 @@ int link_put(pe_link* l, const PutTensor* t, int n_tensors, int items, int bit, 
     p.wire_f16 = l->wire_f16;
     p.is_last = ti == n_tensors - 1 ? 1 : 0;
     p.data_off = off;
-    p.sync_mode = l->sync_mode;
     p.timeout_ns = l->timeout_ns;
     const size_t total = static_cast<size_t>(items) * t[ti].n;
     const bool aligned = (reinterpret_cast<uintptr_t>(t[ti].a) & 15) == 0 &&
@@ -745,22 +692,22 @@ int link_put(pe_link* l, const PutTensor* t, int n_tensors, int items, int bit, 
       PE_REQUIRE(aligned, "pe_link_put: payload tensors must be 16-byte aligned");
       size_t want = (total / 4 + kPutThreads - 1) / kPutThreads;
       // half the SMs move a few MB as fast as all of them and pay half the per-CTA arrival / fence cost
-      const size_t cap = l->grid_cap > 0 ? static_cast<size_t>(l->grid_cap) : static_cast<size_t>((sm_count() + 1) / 2);
+      const size_t cap = static_cast<size_t>((sm_count() + 1) / 2);
       const int grid = static_cast<int>(want < 1 ? 1 : (want > cap ? cap : want));
       link_put_copy_kernel<<<grid, kPutThreads, 0, stream>>>(p);
       PE_CUDA(cudaGetLastError());
       count_launches(1);
     } else if (quant_pack16_applies(bit, t[ti].n, aligned)) {
       // segments: `chunks` per item so that items * chunks ~ the grid; boundaries on multiples of 16 elements
-      const int grid_cap = sm_count() > 16 ? sm_count() - 8 : sm_count();
-      int chunks = items >= grid_cap ? 1 : grid_cap / items;
+      const int max_ctas = sm_count() > 16 ? sm_count() - 8 : sm_count();
+      int chunks = items >= max_ctas ? 1 : max_ctas / items;
       const size_t by_size = (t[ti].n + 4095) / 4096;
       if (static_cast<size_t>(chunks) > by_size) chunks = static_cast<int>(by_size);
       if (chunks > kQMaxChunks) chunks = kQMaxChunks;
       if (chunks < 1) chunks = 1;
       const size_t per = roundup((t[ti].n + chunks - 1) / chunks, 16);
       const int segs = items * chunks;
-      const int grid = segs < grid_cap ? segs : grid_cap;
+      const int grid = segs < max_ctas ? segs : max_ctas;
       const int segs_per_cta = (segs + grid - 1) / grid;
       const size_t cache_bytes = static_cast<size_t>(segs_per_cta) * per * sizeof(float);
       p.chunks = chunks;
@@ -826,14 +773,12 @@ static int launch_get(pe_link* l, const GetArgs& g, size_t work_units, bool may_
   }
   size_t want = (work_units + kGetThreads - 1) / kGetThreads;
   // copies: half the SMs (see link_put); dequantising payloads (the producer announced them at open) want every SM
-  const size_t cap = l->grid_cap > 0 ? static_cast<size_t>(l->grid_cap)
-                                     : static_cast<size_t>(l->quant_hint > 0 ? 2 * sm_count() : (sm_count() + 1) / 2);
+  const size_t cap = static_cast<size_t>(l->quant_hint > 0 ? 2 * sm_count() : (sm_count() + 1) / 2);
   const int grid = static_cast<int>(want < 1 ? 1 : (want > cap ? cap : want));
   const size_t smem = may_decode ? 4096 * sizeof(float) : 0;   // LUT of 2^bit values for bit <= 12
   link_get_kernel<<<grid, kGetThreads, smem, stream>>>(g);
   PE_CUDA(cudaGetLastError());
   count_launches(1);
-  (void)l;
   return PE_OK;
 }
 
@@ -854,7 +799,6 @@ int link_get(pe_link* l, void* dst0, void* dst1, int items, size_t n0, size_t n1
   g.items = items;
   g.n_tensors = n_tensors;
   g.raw = 0;
-  g.sync_mode = l->sync_mode;
   g.timeout_ns = l->timeout_ns;
   return launch_get(l, g, static_cast<size_t>(items) * (n0 + g.n1) / 16, true, prewait, stream);
 }
@@ -870,7 +814,6 @@ int link_get_raw(pe_link* l, void* dst, size_t bytes, cudaStream_t stream, bool 
   g.items = 1;
   g.n_tensors = 1;
   g.raw = 1;
-  g.sync_mode = l->sync_mode;
   g.timeout_ns = l->timeout_ns;
   return launch_get(l, g, bytes / 64, false, prewait, stream);
 }

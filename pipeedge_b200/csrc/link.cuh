@@ -78,7 +78,6 @@ struct PutTensor {
 struct pe_link {
   int fd = -1;               // ticket channel (Unix-domain stream socket); -1 for a host-fed link
   int fd_peer = -1;          // loop-back only: the other end of the socketpair
-  bool own_fd = false;
   int kind = 0;              // 0 = peer (cudaIpc), 1 = loop-back, 2 = host-fed
   bool is_tx = false, is_rx = false;
   size_t slot_bytes = 0;
@@ -97,9 +96,6 @@ struct pe_link {
   size_t quant_work_bytes = 0;
   unsigned long long timeout_ns = 0;
   int wire_f16 = 0;
-  int sync_mode = 0;               // PE_LINK_SYNC bit 0: flags polled with relaxed (volatile) loads; bit 1: one GPU-scope
-                                   // fence per CTA + one system-scope fence by the publishing CTA
-  int grid_cap = 0;                // PE_LINK_GRID_CAP: CTAs of the copy / decode kernels (0 = chosen per kernel)
   int quant_hint = 0;              // bit-width the producer announced at open (0 = raw payloads)
 };
 

@@ -1,14 +1,14 @@
-"""Device time of a link's send + receive pair on a loop-back link under different synchronisation settings
-(PE_LINK_SYNC, PE_LINK_GRID_CAP), each in its own child process; 24 pairs per CUDA graph, CUDA events."""
+"""Device time of a link's send + receive pair on a loop-back link: 24 pairs per CUDA graph, CUDA events."""
+import ctypes
 import os
-import subprocess
 import sys
 
-CHILD = """
-import ctypes, os, sys, torch
-sys.path.insert(0, sys.argv[1])
-from pipeedge_b200 import _lib
-from pipeedge_b200._lib import LIB, check
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from pipeedge_b200 import _lib   # noqa: E402  pylint: disable=wrong-import-position
+from pipeedge_b200._lib import LIB, check   # noqa: E402  pylint: disable=wrong-import-position
+
 dev = torch.device('cuda', 0)
 for label, shape, bit, with_b in (('raw 8x197x768', (8, 197, 768), 0, False), ('raw+add 8x197x768', (8, 197, 768), 0, True),
                                   ('q8 32x198x768 a+b', (32, 198, 768), 8, True), ('raw 32x128x768', (32, 128, 768), 0, False)):
@@ -19,6 +19,7 @@ for label, shape, bit, with_b in (('raw 8x197x768', (8, 197, 768), 0, False), ('
     h = ctypes.c_void_p()
     check(LIB.pe_link_open_local(a.numel() * 4 + 4096, 4, bit, ctypes.byref(h)))
     side = torch.cuda.Stream()
+
     def pair():
         s = torch.cuda.current_stream().cuda_stream
         check(LIB.pe_link_put(h, a.data_ptr(), b.data_ptr() if with_b else None, n, None, None, 0, items, bit,
@@ -44,15 +45,3 @@ for label, shape, bit, with_b in (('raw 8x197x768', (8, 197, 768), 0, False), ('
     us = s.elapsed_time(e) * 1e3 / 240
     print(f"  {label}: {us:.2f} us per put + wait + get", flush=True)
     LIB.pe_link_close(h)
-"""
-root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-if os.environ.get('PE_ONLY_DEFAULT'):     # the library's defaults only
-    print("library defaults (PE_LINK_SYNC=2, copies on half the SMs)", flush=True)
-    env = {k: v for k, v in os.environ.items() if k not in ('PE_LINK_SYNC', 'PE_LINK_GRID_CAP')}
-    subprocess.run([sys.executable, '-c', CHILD, root], env=env, check=False)
-    sys.exit(0)
-for sync in ('0', '1', '2', '3'):
-    for cap in ('0', '74', '37'):
-        print(f"PE_LINK_SYNC={sync} PE_LINK_GRID_CAP={cap}", flush=True)
-        subprocess.run([sys.executable, '-c', CHILD, root], env=dict(os.environ, PE_LINK_SYNC=sync, PE_LINK_GRID_CAP=cap),
-                       check=False)

@@ -50,6 +50,19 @@ def test_no_gpu_means_loud_failure_not_fallback():
         EncoderStage('vit', hf_config(spec), 1, 4, synth_weights(spec), spec.tokens)
 
 
+def test_hop_nccl_is_loaded_with_torch(monkeypatch):
+    """The thread path sends CUDA payloads only through `pe_hop`, which needs nothing but a loadable libnccl.so.2: a
+    CUDA build of torch lists it as a NEEDED library, so any process that imported torch has it. Without it a GPU
+    process refuses to open a hop instead of picking another data plane."""
+    from pipeedge_b200 import _lib
+    from pipeedge_b200.comm import p2p
+    assert _lib.LIB.pe_hop_available() == 1
+    monkeypatch.setattr(torch.cuda, 'is_available', lambda: True)
+    monkeypatch.setattr(_lib.LIB, 'pe_hop_available', lambda: 0)
+    with pytest.raises(RuntimeError, match=r'libnccl\.so\.2'):
+        p2p._native_lib()   # pylint: disable=protected-access
+
+
 def test_clamp_factor_matches_scipy_lambertw():
     from scipy.special import lambertw
     from pipeedge_b200 import _lib
