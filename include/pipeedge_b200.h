@@ -325,6 +325,15 @@ int pe_debug_gemm_trace(void* buf);
  * with `epilogue`: out6 = {cluster_m, cluster_n, block_n, ring stages, tiles, CTAs}. */
 int pe_debug_gemm_plan(int m, int n, int k, int epilogue, int* out6);
 
+/* Host-only: how pe_link_put would ship one tensor of `items` x `n` f32 values at `bit` bits (`aligned`: its a / b are
+ * 16-byte aligned) on the current device (132 SMs without one): out5 = {path, CTAs, chunks per item, elements per
+ * chunk, slice cached}. FUSED = the one-kernel quantise-and-send; its CTA keeps its fp32 slice in shared memory when it
+ * fits in 160 KiB (cached = 1), else pass 2 re-reads it from HBM. STAGED = stand-alone quant kernels + a copy kernel. */
+#define PE_LINK_PATH_COPY 0
+#define PE_LINK_PATH_FUSED 1
+#define PE_LINK_PATH_STAGED 2
+int pe_debug_link_put_plan(int items, size_t n, int bit, int aligned, int* out5);
+
 #ifdef __cplusplus
 }
 #endif

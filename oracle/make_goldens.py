@@ -14,6 +14,9 @@ Fixture contents
 * `quant.npz`: `tensor_encode_outerdim` outputs and `tensor_decode_outerdim` round trips for
   several bit widths, plus the two runtime hooks' clamp thresholds (restated in this script
   without the `monitoring` calls - `runtime.py` itself cannot be imported here, SURVEY.md 8c).
+* `quant_bits.npz` (`python -m oracle.make_goldens quant_bits`): the same for the bit-widths `quant.npz` leaves out
+  (1, 7, 9, 11, 12, 13, 14, 15) on normal, outlier, rounding-tie and every-code inputs, through the reference's
+  `basic_op` and `clamp_op` only (no constant items: the reference asserts on them).
 * `adaptive.json` (`python -m oracle.make_goldens adaptive`): outputs of the reference's adaptive-QuantPipe policy
   code (`<checkout>/utils/{quant,controller}.py`): `constrain_max_bitwidth` over a grid, Kalman-filter and
   bit-width-controller traces for fixed measurement sequences.
@@ -134,6 +137,45 @@ def golden_quant():
     print('quant done')
 
 
+QUANT_BITS = (1, 7, 9, 11, 12, 13, 14, 15)
+
+
+def golden_quant_bits():
+    """Stored per bit b and input kind k: x_k_b, alpha_k_b (the clamp's threshold), comm / shape / scale / shift /
+    bit_k_b and dec_k_b, as `golden_quant`."""
+    _, _, basic_op, clamp_op = _ref()
+    out = {}
+    gen = torch.Generator().manual_seed(17)
+    for bit in QUANT_BITS:
+        lv = (1 << bit) - 1
+        xs = {'normal': torch.randn(3, 7, 41, generator=gen) * 1.3 + 0.1,
+              'outliers': torch.randn(4, 300, generator=gen) * 1.3 + 0.1}
+        xs['outliers'][0, :3] = torch.tensor([40.0, -35.0, 12.0])
+        # ties: values v with lv * fp32(v / S) == k + 1/2 in fp32 (S = lv), the rest of the item spanning [0, S]; the
+        # second item (+-100 S) keeps the Laplace threshold above S
+        s = np.float32(lv)
+        ties = [np.float32(0.0), s] + [np.float32(k + 0.5) for k in range(min(lv, 300))
+                                      if float(np.float32(lv) * np.float32(np.float32(k + 0.5) / s)) == k + 0.5]
+        ramp = np.arange(lv + 1, dtype=np.float32)
+        for kind, vals in (('ties', ties), ('ramp', ramp)):
+            vals = np.asarray(vals, dtype=np.float32)
+            perm = torch.randperm(len(vals), generator=gen).numpy()
+            guard = np.resize(np.array([-100 * s, 100 * s], np.float32), len(vals))
+            xs[kind] = torch.from_numpy(np.stack([vals[perm], guard]))
+        for kind, x in xs.items():
+            key = f"{kind}_{bit}"
+            out[f"x_{key}"] = x.numpy()
+            clamp = clamp_op.clamp_banner2019_laplace if x.min() < 0.2 else clamp_op.clamp_banner2019_gelu
+            xc = clamp(x, bit)
+            out[f"alpha_{key}"] = np.float32(xc.abs().max().item())
+            enc = basic_op.tensor_encode_outerdim(xc, bit)
+            for nm, t in zip(('comm', 'shape', 'scale', 'shift', 'bit'), enc):
+                out[f"{nm}_{key}"] = t.numpy()
+            out[f"dec_{key}"] = basic_op.tensor_decode_outerdim(enc).numpy()
+    np.savez_compressed(os.path.join(OUT, "quant_bits.npz"), **out)
+    print('quant_bits done')
+
+
 def _ref_utils():
     """The reference's top-level `utils` package, imported under another name (this repo has its own `utils`)."""
     import importlib.util   # pylint: disable=import-outside-toplevel
@@ -251,12 +293,16 @@ def main():
     if sys.argv[1:] == ['sched']:
         golden_sched()
         return
+    if sys.argv[1:] == ['quant_bits']:
+        golden_quant_bits()
+        return
     if sys.argv[1:] == ['vit-large']:
         golden_full('google/vit-large-patch16-224', 2, (24, 48, 72, 96))
         return
     golden_adaptive()
     golden_sched()
     golden_quant()
+    golden_quant_bits()
     for name in ('test/vit-tiny', 'test/deit-tiny', 'test/bert-tiny', 'test/vit-huge-tiny'):
         golden_tiny(name)
     golden_full('google/vit-base-patch16-224', 2, (2, 24, 48))

@@ -4,7 +4,8 @@ NumPy restatement of `pipeedge/quantization/basic_op.py` and `clamp_op.py`, plus
 hooks that drive them (`runtime.py:73-119`). Integer codes, scales and shifts produced here are
 the bit-exact target for the CUDA path.
 """
-from typing import List, Sequence, Tuple
+import math
+from typing import List, Optional, Sequence, Tuple
 import numpy as np
 import torch
 from scipy.special import lambertw
@@ -20,13 +21,14 @@ def clamp_factor_gelu(bit: int) -> np.float32:
     return np.float32(lambertw(3.0 * 4.0 ** (bit + 1)).real)
 
 
-def clamp_alpha(tensor: torch.Tensor, bit: int) -> Tuple[np.float32, str]:
+def clamp_alpha(tensor: torch.Tensor, bit: int, kind: Optional[str] = None) -> Tuple[np.float32, str]:
     """Clamp threshold chosen by `forward_hook_quant_encode` (`runtime.py:84`) for a micro-batch.
 
     Laplace (`clamp_op.py:27-33`): alpha = W * sqrt(0.5 * var(x, biased)); GeLU (`:11-19`):
-    var ~= 2 * sum(x^2) / n. All in fp32 after torch's own reductions.
+    var ~= 2 * sum(x^2) / n. All in fp32 after torch's own reductions. `kind` = 'laplace' / 'gelu' calls that clamp
+    function directly (PE_CLAMP_LAPLACE / PE_CLAMP_GELU) instead of choosing by min(x) < 0.2.
     """
-    if tensor.min() < 0.2:
+    if kind == 'laplace' or (kind is None and tensor.min() < 0.2):
         variance = torch.var(tensor, unbiased=False)
         factor, kind = clamp_factor_laplace(bit), 'laplace'
     else:
@@ -64,11 +66,21 @@ def quant_codes(item: np.ndarray, bit: int) -> Tuple[np.ndarray, np.float32, np.
     shift = item.min()
     centred = item - shift
     scale = centred.max()
+    if scale == 0:
+        return constant_item_codes(item)
     rescale = centred / scale
     assert np.all(rescale >= 0) and np.all(rescale <= 1)   # `_quant_op` asserts (NaN if scale == 0)
     levels = (1 << bit) - 1
     codes = np.around(levels * rescale).astype(np.uint32)
     return codes, np.float32(scale), np.float32(shift)
+
+
+def constant_item_codes(item: np.ndarray) -> Tuple[np.ndarray, np.float32, np.float32]:
+    """A constant item (scale 0; also an item the clamp maps entirely onto +-alpha): zero codes, scale 0, shift = the
+    value, so that decoding (0 * 0 + shift) gives the value back. The reference trips its NaN assert here
+    (`basic_op.py:12-13`); this is the deliberate deviation of DESIGN.md section 2, restated for the tests."""
+    item = np.asarray(item, dtype=np.float32)
+    return np.zeros(item.shape, dtype=np.uint32), np.float32(0.0), np.float32(item.min())
 
 
 def pack_codes(codes: np.ndarray, bit: int) -> np.ndarray:
@@ -140,6 +152,16 @@ def hook_encode(output, bit: int) -> tuple:
             tensor = clamp(tensor, bit)
         comm += tensor_encode_outerdim(tensor, bit)
     return tuple(comm)
+
+
+def encode_given_alpha(x: torch.Tensor, bit: int, alpha) -> tuple:
+    """`hook_encode` of one tensor with the clamp threshold given instead of computed: x clamped to [-alpha, alpha]
+    (no clamp when alpha is +inf), then `tensor_encode_outerdim`. The GeLU branch's threshold depends in its last bits
+    on the fp32 summation order (`clamp_alpha`), so a kernel's codes are held to the oracle at the kernel's own alpha."""
+    a = float(np.float32(alpha))
+    if not math.isinf(a):
+        x = x.clamp(min=-a, max=a)
+    return tuple(tensor_encode_outerdim(x, bit))
 
 
 def hook_decode(tensors: tuple):

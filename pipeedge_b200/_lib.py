@@ -17,6 +17,7 @@ PE_EPI_STATIC_W = 0x100   # OR-able flag: W is a model weight (not produced by p
 PE_CLAMP_NONE, PE_CLAMP_AUTO, PE_CLAMP_LAPLACE, PE_CLAMP_GELU = range(4)
 PE_STAGE_DEFER_ADD = 2        # OR-able into pe_stage_forward's use_graph (eager only)
 PE_LINK_HEADER_BYTES = 16384
+PE_LINK_PATH_COPY, PE_LINK_PATH_FUSED, PE_LINK_PATH_STAGED = range(3)   # pe_debug_link_put_plan
 PE_ABI_VERSION = 2
 
 
@@ -107,6 +108,7 @@ SYMBOLS = {
                                POINTER(c_ulonglong)]),
     'pe_debug_gemm_trace': (c_int, [c_void_p]),
     'pe_debug_gemm_plan': (c_int, [c_int] * 4 + [c_void_p]),
+    'pe_debug_link_put_plan': (c_int, [c_int, c_size_t, c_int, c_int, c_void_p]),
     'pe_debug_linear_simt': (c_int, [c_void_p] * 5 + [c_int] * 4 + [c_void_p]),
 }
 

@@ -304,15 +304,26 @@ __global__ void add_f32_kernel(const float* __restrict__ a, const float* b, floa
   }
 }
 
+// The same, one float per thread, for operands that are not 16-byte aligned (a link payload's a / b may start anywhere).
+__global__ void add_f32_scalar_kernel(const float* __restrict__ a, const float* b, float* out, size_t n) {
+  const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n; i += stride) out[i] = a[i] + b[i];
+}
+
 int add_impl(const void* a, const void* b, void* out, size_t n, cudaStream_t stream) {
   PE_REQUIRE(a && b && out && (n & 3) == 0, "pe_add: bad arguments");
-  const size_t n4 = n >> 2;
-  size_t want = (n4 + 255) / 256;
+  const bool vec = ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(out)) & 15) == 0;
+  const size_t units = vec ? n >> 2 : n;
+  size_t want = (units + 255) / 256;
   const int grid = static_cast<int>(want < 1 ? 1 : (want > static_cast<size_t>(kNumSMs) * 8 ? kNumSMs * 8 : want));
   static bool configured = false;
   if (!configured) { prefer_max_shared(add_f32_kernel); configured = true; }
-  add_f32_kernel<<<grid, 256, 0, stream>>>(static_cast<const float*>(a), static_cast<const float*>(b),
-                                           static_cast<float*>(out), n4);
+  if (vec)
+    add_f32_kernel<<<grid, 256, 0, stream>>>(static_cast<const float*>(a), static_cast<const float*>(b),
+                                             static_cast<float*>(out), units);
+  else
+    add_f32_scalar_kernel<<<grid, 256, 0, stream>>>(static_cast<const float*>(a), static_cast<const float*>(b),
+                                                    static_cast<float*>(out), n);
   PE_CUDA(cudaGetLastError());
   count_launches(1);
   return PE_OK;

@@ -662,6 +662,54 @@ static size_t wire_bytes(const pe_link* l, int items, size_t n, int bit) {
   return static_cast<size_t>(items) * quant_words(n, bit) * 4;
 }
 
+// How link_put ships one tensor of `items` x `n` values at `bit` bits on a GPU with `sms` SMs. `aligned`: a (and b)
+// are 16-byte aligned. The one place that decides it: link_put launches what this returns, and
+// pe_debug_link_put_plan reports it.
+struct PutPlan {
+  int path;        // PE_LINK_PATH_*
+  int grid;        // CTAs of the send kernel
+  int chunks;      // fused: segments per item
+  size_t per;      // fused: elements per segment (multiple of 16)
+  int cache;       // fused: the CTA's fp32 slice stays in shared memory between the passes (else pass 2 re-reads HBM)
+  size_t smem;     // fused: dynamic shared memory
+};
+
+static PutPlan plan_put(int items, size_t n, int bit, bool aligned, int sms) {
+  PutPlan pl = {};
+  const size_t total = static_cast<size_t>(items) * n;
+  if (bit == 0) {
+    pl.path = PE_LINK_PATH_COPY;
+    const size_t want = (total / 4 + kPutThreads - 1) / kPutThreads;
+    // half the SMs move a few MB as fast as all of them and pay half the per-CTA arrival / fence cost
+    const size_t cap = static_cast<size_t>((sms + 1) / 2);
+    pl.grid = static_cast<int>(want < 1 ? 1 : (want > cap ? cap : want));
+  } else if (quant_pack16_applies(bit, n, aligned)) {
+    pl.path = PE_LINK_PATH_FUSED;
+    // segments: `chunks` per item so that items * chunks ~ the grid; boundaries on multiples of 16 elements
+    const int max_ctas = sms > 16 ? sms - 8 : sms;
+    int chunks = items >= max_ctas ? 1 : max_ctas / items;
+    const size_t by_size = (n + 4095) / 4096;
+    if (static_cast<size_t>(chunks) > by_size) chunks = static_cast<int>(by_size);
+    if (chunks > kQMaxChunks) chunks = kQMaxChunks;
+    if (chunks < 1) chunks = 1;
+    pl.chunks = chunks;
+    pl.per = roundup((n + chunks - 1) / chunks, 16);
+    const int segs = items * chunks;
+    pl.grid = segs < max_ctas ? segs : max_ctas;
+    const int segs_per_cta = (segs + pl.grid - 1) / pl.grid;
+    const size_t cache_bytes = roundup(static_cast<size_t>(segs_per_cta) * pl.per * sizeof(float), 128);
+    pl.cache = cache_bytes <= kQuantCacheBytes ? 1 : 0;
+    pl.smem = pl.cache ? cache_bytes : 0;   // whole swizzle groups of 8 float4
+  } else {
+    // generic bit-widths / shapes: the stand-alone kernels quantise into local staging, one kernel ships it
+    pl.path = PE_LINK_PATH_STAGED;
+    const size_t bytes = static_cast<size_t>(items) * quant_words(n, bit) * 4;
+    const size_t want = (bytes / 4 + kPutThreads - 1) / kPutThreads;
+    pl.grid = static_cast<int>(want < 1 ? 1 : (want > static_cast<size_t>(2 * sms) ? 2 * sms : want));
+  }
+  return pl;
+}
+
 int link_put(pe_link* l, const PutTensor* t, int n_tensors, int items, int bit, int clamp, cudaStream_t stream) {
   PE_REQUIRE(l != nullptr && l->is_tx, "pe_link_put: not the producer end of a link");
   PE_REQUIRE(n_tensors >= 1 && n_tensors <= 2 && items > 0 && items <= kLinkMaxItems,
@@ -688,44 +736,27 @@ int link_put(pe_link* l, const PutTensor* t, int n_tensors, int items, int bit, 
     const size_t total = static_cast<size_t>(items) * t[ti].n;
     const bool aligned = (reinterpret_cast<uintptr_t>(t[ti].a) & 15) == 0 &&
                          (t[ti].b == nullptr || (reinterpret_cast<uintptr_t>(t[ti].b) & 15) == 0);
-    if (bit == 0) {
+    const PutPlan pl = plan_put(items, t[ti].n, bit, aligned, sm_count());
+    if (pl.path == PE_LINK_PATH_COPY) {
       PE_REQUIRE(aligned, "pe_link_put: payload tensors must be 16-byte aligned");
-      size_t want = (total / 4 + kPutThreads - 1) / kPutThreads;
-      // half the SMs move a few MB as fast as all of them and pay half the per-CTA arrival / fence cost
-      const size_t cap = static_cast<size_t>((sm_count() + 1) / 2);
-      const int grid = static_cast<int>(want < 1 ? 1 : (want > cap ? cap : want));
-      link_put_copy_kernel<<<grid, kPutThreads, 0, stream>>>(p);
+      link_put_copy_kernel<<<pl.grid, kPutThreads, 0, stream>>>(p);
       PE_CUDA(cudaGetLastError());
       count_launches(1);
-    } else if (quant_pack16_applies(bit, t[ti].n, aligned)) {
-      // segments: `chunks` per item so that items * chunks ~ the grid; boundaries on multiples of 16 elements
-      const int max_ctas = sm_count() > 16 ? sm_count() - 8 : sm_count();
-      int chunks = items >= max_ctas ? 1 : max_ctas / items;
-      const size_t by_size = (t[ti].n + 4095) / 4096;
-      if (static_cast<size_t>(chunks) > by_size) chunks = static_cast<int>(by_size);
-      if (chunks > kQMaxChunks) chunks = kQMaxChunks;
-      if (chunks < 1) chunks = 1;
-      const size_t per = roundup((t[ti].n + chunks - 1) / chunks, 16);
-      const int segs = items * chunks;
-      const int grid = segs < max_ctas ? segs : max_ctas;
-      const int segs_per_cta = (segs + grid - 1) / grid;
-      const size_t cache_bytes = static_cast<size_t>(segs_per_cta) * per * sizeof(float);
-      p.chunks = chunks;
-      p.per = per;
-      p.cache = roundup(cache_bytes, 128) <= kQuantCacheBytes ? 1 : 0;
+    } else if (pl.path == PE_LINK_PATH_FUSED) {
+      p.chunks = pl.chunks;
+      p.per = pl.per;
+      p.cache = pl.cache;
       p.factor_laplace = clamp_factor(bit, 0);
       p.factor_gelu = clamp_factor(bit, 1);
-      const size_t smem = p.cache ? roundup(cache_bytes, 128) : 0;   // whole swizzle groups of 8 float4
       switch (bit) {
-        case 2: link_put_quant_kernel<2><<<grid, kPutThreads, smem, stream>>>(p); break;
-        case 4: link_put_quant_kernel<4><<<grid, kPutThreads, smem, stream>>>(p); break;
-        case 8: link_put_quant_kernel<8><<<grid, kPutThreads, smem, stream>>>(p); break;
-        default: link_put_quant_kernel<16><<<grid, kPutThreads, smem, stream>>>(p); break;
+        case 2: link_put_quant_kernel<2><<<pl.grid, kPutThreads, pl.smem, stream>>>(p); break;
+        case 4: link_put_quant_kernel<4><<<pl.grid, kPutThreads, pl.smem, stream>>>(p); break;
+        case 8: link_put_quant_kernel<8><<<pl.grid, kPutThreads, pl.smem, stream>>>(p); break;
+        default: link_put_quant_kernel<16><<<pl.grid, kPutThreads, pl.smem, stream>>>(p); break;
       }
       PE_CUDA(cudaGetLastError());
       count_launches(1);
     } else {
-      // generic bit-widths / shapes: the stand-alone kernels quantise into local staging, one kernel ships it
       const float* x = t[ti].a;
       const size_t codes_bytes = roundup(bytes, 256);
       const size_t need = codes_bytes + 2 * roundup(items * sizeof(float), 256) + 256 + roundup(quant_workspace_bytes(items, t[ti].n), 256);
@@ -750,9 +781,7 @@ int link_put(pe_link* l, const PutTensor* t, int n_tensors, int items, int bit, 
       p.staged_shift = shift;
       p.staged_alpha = alpha;
       p.staged_bytes = bytes;
-      size_t want = (bytes / 4 + kPutThreads - 1) / kPutThreads;
-      const int grid = static_cast<int>(want < 1 ? 1 : (want > static_cast<size_t>(2 * sm_count()) ? 2 * sm_count() : want));
-      link_put_staged_kernel<<<grid, kPutThreads, 0, stream>>>(p);
+      link_put_staged_kernel<<<pl.grid, kPutThreads, 0, stream>>>(p);
       PE_CUDA(cudaGetLastError());
       count_launches(1);
     }
@@ -1132,6 +1161,20 @@ int pe_link_debug_read(pe_link* link, unsigned long long seq, size_t offset, voi
   PE_CUDA(cudaDeviceSynchronize());
   const uint8_t* src = link->rx.ring + (seq % static_cast<unsigned long long>(link->n_slots)) * link->slot_bytes + offset;
   PE_CUDA(cudaMemcpy(host_dst, src, bytes, cudaMemcpyDeviceToHost));
+  return PE_OK;
+}
+
+// Host-only: how pe_link_put would ship one tensor on this device (kNumSMs SMs when there is none).
+int pe_debug_link_put_plan(int items, size_t n, int bit, int aligned, int* out5) {
+  using namespace pe;
+  PE_REQUIRE(out5 != nullptr && items > 0 && items <= kLinkMaxItems && n > 0 && bit >= 0 && bit <= 16,
+             "pe_debug_link_put_plan: bad arguments");
+  const PutPlan pl = plan_put(items, n, bit, aligned != 0, sm_count());
+  out5[0] = pl.path;
+  out5[1] = pl.grid;
+  out5[2] = pl.chunks;
+  out5[3] = static_cast<int>(pl.per);
+  out5[4] = pl.cache;
   return PE_OK;
 }
 

@@ -150,3 +150,28 @@ def test_gelu_clamp_threshold_of_the_reference_is_not_a_single_number():
     # what the CUDA kernel computes: the fp64 sum of fp32-rounded squares, rounded to fp32
     ours = float(np.float32((x * x).double().sum()))
     assert lo - 2 * ulp <= ours <= hi + 2 * ulp
+
+
+QB = np.load(os.path.join(GOLDEN, 'quant_bits.npz'))
+
+
+@pytest.mark.parametrize('kind', ['normal', 'outliers', 'ties', 'ramp'])
+@pytest.mark.parametrize('bit', [1, 7, 9, 11, 12, 13, 14, 15])
+def test_quant_remaining_bit_widths_bit_exact(kind, bit):
+    """The bit-widths `quant.npz` leaves out, made by the reference's `basic_op` + `clamp_op`: the oracle reproduces
+    every wire byte, scale, shift and decoded value, and the clamp threshold wherever the clamp bites."""
+    key = f"{kind}_{bit}"
+    x = torch.from_numpy(QB[f"x_{key}"])
+    enc = oq.hook_encode(x, bit)
+    for nm, t in zip(('comm', 'shape', 'scale', 'shift', 'bit'), enc):
+        want = QB[f"{nm}_{key}"]
+        assert t.numpy().dtype == want.dtype, nm
+        np.testing.assert_array_equal(t.numpy(), want, err_msg=nm)
+    np.testing.assert_array_equal(oq.hook_decode(enc).numpy(), QB[f"dec_{key}"])
+    alpha, kind_ = oq.clamp_alpha(x, bit)
+    assert kind_ == 'laplace'
+    if x.abs().max() > alpha:
+        assert alpha == QB[f"alpha_{key}"]
+    if kind == 'ramp':
+        codes = oq.unpack_codes(enc[0][0].numpy().view(np.uint32), x.shape[1], bit)
+        assert set(codes.tolist()) == set(range(1 << bit))
