@@ -295,6 +295,34 @@ int pe_pipe_timing_reset(pe_pipe* pipe);
 int pe_pipe_timing(pe_pipe* pipe, float* compute_ms, float* results_ms, unsigned long long* launches,
                    unsigned long long* kernels);
 
+/* Per-micro-batch device timestamps. With stamps on, graphs captured from then on carry one-thread kernels that read
+ * %globaltimer (ns) into a ring of PE_PIPE_STAMP_DEPTH records in mapped host memory; the graphs still take no per-launch
+ * arguments (device-resident counters pick the record). Turning them on or off makes every graph captured the other
+ * way count as missing: the next payload of its shape captures again. Graphs captured without stamps are exactly the
+ * graphs of a pipe that never had them. */
+#define PE_PIPE_STAMP_DEPTH 256
+#define PE_STAMP_OVERLAPPED 1   /* the send ran as its own graph, overlapping the next micro-batch */
+#define PE_STAMP_FUSED 2        /* a tensor went through the fused quantise-and-send kernel */
+#define PE_STAMP_STAGED 4       /* a tensor went through the stand-alone encode kernels + a shipping kernel */
+typedef struct pe_pipe_record {
+  unsigned long long index;        /* records of this pipe before this one */
+  unsigned long long t_start;      /* graph start, before the receive */
+  unsigned long long t_got;        /* receive (and dequantise) done */
+  unsigned long long t_stage;      /* the stage's last kernel done */
+  unsigned long long t_send_start; /* send start (= t_stage when the send is inside the main graph) */
+  unsigned long long t_encoded;    /* staged send: its stand-alone encode kernels done; else 0 */
+  unsigned long long t_send_end;   /* send done: the payload is published to the consumer */
+  unsigned long long bytes_out;    /* payload bytes the send wrote (pe_link_payload_bytes, summed over its tensors) */
+  int items;                       /* micro-batch size */
+  int bit_out;                     /* bit-width the send quantised to (0 = raw values) */
+  int bit_in;                      /* bit-width of the payload the receive consumed, from its slot header; -1: host-fed */
+  int flags;                       /* PE_STAMP_* */
+} pe_pipe_record;
+int pe_pipe_enable_stamps(pe_pipe* pipe, int on);
+/* Non-blocking: copy up to `max` records completed since the previous call into `out` (oldest first; *n of them) and add
+ * to *dropped the records that were overwritten before they could be read (a reader a whole ring behind). */
+int pe_pipe_drain_stamps(pe_pipe* pipe, pe_pipe_record* out, int max, int* n, unsigned long long* dropped);
+
 /* ---- Inter-stage hop over NCCL (generic payloads) -----------------------------------------------
  * Replaces `TensorSendThread.run` / `TensorRecvThread.run` + `_send_tensor` / `_recv_tensor`
  * (`p2p/__init__.py:96-258`) for the device tensors of a payload: one call per payload and side, over a
@@ -333,6 +361,10 @@ int pe_debug_gemm_plan(int m, int n, int k, int epilogue, int* out6);
 #define PE_LINK_PATH_FUSED 1
 #define PE_LINK_PATH_STAGED 2
 int pe_debug_link_put_plan(int items, size_t n, int bit, int aligned, int* out5);
+/* Host-only: bytes a put of one [items, n] tensor at `bit` bits writes - the f32 values (f16 with `wire_f16`), or the
+ * packed codes plus the per-item f32 scale and shift. With wire_f16 == 0 it equals what the Python-thread path moves for
+ * the same tensor (its CUDA tensors: the values, or codes + scale + shift). 0 for invalid arguments. */
+size_t pe_link_payload_bytes(int items, size_t n, int bit, int wire_f16);
 
 #ifdef __cplusplus
 }

@@ -19,6 +19,8 @@ PE_STAGE_DEFER_ADD = 2        # OR-able into pe_stage_forward's use_graph (eager
 PE_LINK_HEADER_BYTES = 16384
 PE_LINK_PATH_COPY, PE_LINK_PATH_FUSED, PE_LINK_PATH_STAGED = range(3)   # pe_debug_link_put_plan
 PE_ABI_VERSION = 2
+PE_PIPE_STAMP_DEPTH = 256
+PE_STAMP_OVERLAPPED, PE_STAMP_FUSED, PE_STAMP_STAGED = 1, 2, 4   # pe_pipe_record.flags
 
 
 class PipeEdgeB200Error(RuntimeError):
@@ -35,6 +37,13 @@ class StageDesc(Structure):
     """`pe_stage_desc`."""
     _fields_ = [('family', c_int), ('hidden', c_int), ('heads', c_int), ('inter', c_int), ('tokens', c_int),
                 ('eps', c_float), ('layer_start', c_int), ('layer_end', c_int), ('max_ubatch', c_int)]
+
+
+class PipeRecord(Structure):
+    """`pe_pipe_record`: one micro-batch's device timestamps (%globaltimer ns) on a pipe with stamps on."""
+    _fields_ = [(n, c_ulonglong) for n in ('index', 't_start', 't_got', 't_stage', 't_send_start', 't_encoded',
+                                           't_send_end', 'bytes_out')] + \
+               [(n, c_int) for n in ('items', 'bit_out', 'bit_in', 'flags')]
 
 
 # name -> (restype, argtypes); every symbol declared in include/pipeedge_b200.h
@@ -106,6 +115,9 @@ SYMBOLS = {
     'pe_pipe_timing_reset': (c_int, [c_void_p]),
     'pe_pipe_timing': (c_int, [c_void_p, POINTER(c_float), POINTER(c_float), POINTER(c_ulonglong),
                                POINTER(c_ulonglong)]),
+    'pe_pipe_enable_stamps': (c_int, [c_void_p, c_int]),
+    'pe_pipe_drain_stamps': (c_int, [c_void_p, POINTER(PipeRecord), c_int, POINTER(c_int), POINTER(c_ulonglong)]),
+    'pe_link_payload_bytes': (c_size_t, [c_int, c_size_t, c_int, c_int]),
     'pe_debug_gemm_trace': (c_int, [c_void_p]),
     'pe_debug_gemm_plan': (c_int, [c_int] * 4 + [c_void_p]),
     'pe_debug_link_put_plan': (c_int, [c_int, c_size_t, c_int, c_int, c_void_p]),

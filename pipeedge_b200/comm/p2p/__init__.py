@@ -787,9 +787,9 @@ class DistP2pPipelineStage:
             return False
         if work_cb is None or not shard_is_native(work_cb):
             return False
-        if any(thr._pre_hooks or thr._post_hooks or getattr(thr, '_timing_hooks', None)   # pylint: disable=protected-access
+        if any(thr._pre_hooks or thr._post_hooks   # pylint: disable=protected-access
                for thr in self._threads.values() if isinstance(thr, AbstractTensorExchangeThread)):
-            return False   # user hooks run on the Python exchange threads
+            return False   # user hooks run on the Python exchange threads (send-timing hooks do not: device timestamps)
         if (rank_src is None) != (rank_dst is None):
             return False
         if results_cb is not None and not work_cb.shard_config.is_first:
@@ -838,6 +838,9 @@ class DistP2pPipelineStage:
             if work_cb is not None:
                 from ._native import NativeStage   # pylint: disable=import-outside-toplevel
                 self._native = NativeStage(rank_src, rank_dst, work_cb, results_cb)
+                send = self._threads.get('send')
+                for hook, args in (send._timing_hooks if send is not None else ()):   # pylint: disable=protected-access
+                    self._native.add_send_timing_hook(hook, args)   # registered before init(): stamps from the start
                 self._native.init(DistP2pContext.connect_to, DistP2pContext.accept_from)
             return
         # Open this rank's hops in ascending order of the hop's SENDER rank before any thread runs. Opening blocks
@@ -903,8 +906,16 @@ class DistP2pPipelineStage:
         """Register `hook(mbits, seconds, *args)`, called with each payload's DEVICE-side transfer time (CUDA events
         around the hop's NCCL sends). The send post hook above fires when a send is enqueued, not when it has
         finished, so bandwidth-driven policies (`runtime.py:121-216` in the reference) read this instead. No
-        reference equivalent: there the blocking send itself is timed on the host."""
-        self._no_hooks_on_native()
+        reference equivalent: there the blocking send itself is timed on the host.
+
+        Legal before or after `init()` on the native pipeline too: there `seconds` is the send's duration from the
+        graph's device timestamps (send start -> payload published; it includes waiting for a free slot, like the
+        NCCL send includes waiting for the receiver) and `mbits` is what the thread path reports for the same payload."""
+        if self._native is not None:
+            self._native.add_send_timing_hook(hook, args)
+            return
+        if self._native_world:
+            return   # idle rank: it sends nothing
         thr = self._threads.get('send')
         if thr is not None:
             thr.register_timing_hook(hook, args)

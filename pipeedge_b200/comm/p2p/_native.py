@@ -12,13 +12,18 @@ Activations cross hops as peer-memory stores synchronised by device-polled flags
 quantisation (`-q`, the shard's `quant_bit` buffer) is fused into the send kernel and undone by the receive kernel, so
 the Python quantisation hooks (`runtime.py:73-119`) are represented by those kernels rather than called. Python runs
 once per (micro-batch size, sequence length): to capture the graph.
+
+Per-micro-batch timing: with stamps on (a shard hook that asks for records, or a send-timing hook), the graphs also
+write device timestamps into a ring of records in host memory (`pe_pipe_enable_stamps`); a drain thread turns each
+completed record into calls of the stage's record consumers and send-timing hooks, off the graph-launch path.
 """
 import collections
 import ctypes
 import logging
 import os
 import threading
-from typing import Callable, Optional
+import time
+from typing import Callable, List, NamedTuple, Optional
 import torch
 import torch.distributed as dist
 from ... import _lib
@@ -60,13 +65,93 @@ def hook_is_native(hook) -> bool:
     return bool(flag() if callable(flag) else flag)
 
 
+def _shard_hooks(shard) -> list:
+    return list(getattr(shard, '_forward_hooks', {}).values()) + list(getattr(shard, '_forward_pre_hooks', {}).values())
+
+
 def shard_is_native(shard) -> bool:
     """A native shard whose registered hooks the native pipeline accounts for."""
     from ...models.transformers._shard import GpuTransformerShard   # pylint: disable=import-outside-toplevel
     if not isinstance(shard, GpuTransformerShard):
         return False
-    hooks = list(getattr(shard, '_forward_hooks', {}).values()) + list(getattr(shard, '_forward_pre_hooks', {}).values())
-    return all(hook_is_native(h) for h in hooks)
+    return all(hook_is_native(h) for h in _shard_hooks(shard))
+
+
+def record_consumers(shard) -> List[Callable]:
+    """The per-micro-batch record consumers the shard's hooks ask for: a hook may carry `_pe_records`, a callable
+    `(shard) -> Optional[consumer]`; each consumer is called with every `StampRecord` of the stage."""
+    consumers = []
+    for hook in _shard_hooks(shard):
+        factory = getattr(hook, '_pe_records', None)
+        consumer = factory(shard) if factory is not None else None
+        if consumer is not None:
+            consumers.append(consumer)
+    return consumers
+
+
+class StampRecord(NamedTuple):
+    """One micro-batch of a stage on the native pipeline, as its graph timestamped it (`pe_pipe_record`; times are
+    device %globaltimer nanoseconds). `t_send_start == t_stage` when the send runs inside the main graph; `t_encoded`
+    is 0 unless the send took the staged path (stand-alone encode kernels, then a shipping kernel). `bit_in` is -1 on
+    the data rank (its input is fed by the host)."""
+    index: int
+    items: int
+    bit_out: int
+    bit_in: int
+    bytes_out: int
+    flags: int
+    t_start: int
+    t_got: int
+    t_stage: int
+    t_send_start: int
+    t_encoded: int
+    t_send_end: int
+
+    @classmethod
+    def from_c(cls, rec: _lib.PipeRecord) -> 'StampRecord':
+        """Copy a `pe_pipe_record`."""
+        return cls(**{name: getattr(rec, name) for name in cls._fields})
+
+    @property
+    def send_mbits(self) -> float:
+        """The payload in Mbit, as the Python-thread path's send-timing hook reports it (bytes * 8e-6)."""
+        return self.bytes_out * 8e-6
+
+    @property
+    def send_seconds(self) -> float:
+        """Device time of the send: send start -> the payload published to the consumer."""
+        return (self.t_send_end - self.t_send_start) * 1e-9
+
+
+class RecordDrain:
+    """Reader side of a pipe's timestamp ring: `poll()` drains what has completed (non-blocking) and hands each record to
+    `dispatch`; `dropped` counts records overwritten before they were read. `drain_fn(buf, max, n, dropped)` is
+    `pe_pipe_drain_stamps` bound to one pipe (injectable for tests)."""
+
+    def __init__(self, drain_fn: Callable, dispatch: Callable[[StampRecord], None], batch: int = 64):
+        self._drain_fn = drain_fn
+        self._dispatch = dispatch
+        self._buf = (_lib.PipeRecord * batch)()
+        self.dropped = 0
+        self.records = 0
+
+    def poll(self) -> int:
+        """Dispatch every completed record; returns how many."""
+        total = 0
+        n, dropped = ctypes.c_int(), ctypes.c_ulonglong()
+        while True:
+            dropped.value = 0
+            check(self._drain_fn(self._buf, len(self._buf), ctypes.byref(n), ctypes.byref(dropped)))
+            if dropped.value:
+                self.dropped += dropped.value
+                logger.warning("native pipeline: %d timestamp records were overwritten before they were read",
+                               dropped.value)
+            for i in range(n.value):
+                self._dispatch(StampRecord.from_c(self._buf[i]))
+            total += n.value
+            self.records += n.value
+            if n.value < len(self._buf):
+                return total
 
 
 class NativeStage:
@@ -95,6 +180,11 @@ class NativeStage:
         self._quant_key, self._quant_val = None, 0
         self._stream = None
         self._copy_stream = None
+        self._record_cbs = record_consumers(shard)   # per-micro-batch record consumers (from the shard's hooks)
+        self._send_hooks = []                          # (hook, args): hook(mbits, seconds, *args) per payload sent
+        self._drain = None                             # RecordDrain once stamps are on
+        self._drain_stop = threading.Event()
+        self._drain_thread = None
 
     # ------------------------------------------------------------------ set-up
     def _open_link(self, sock, is_producer: bool, payload_bytes: int) -> ctypes.c_void_p:
@@ -159,8 +249,58 @@ class NativeStage:
             thr = threading.Thread(target=self._guard, args=(self._results_loop,), daemon=True, name='pe-results')
         else:
             thr = threading.Thread(target=self._guard, args=(self._run_loop,), daemon=True, name='pe-stage')
+        if self._record_cbs or self._send_hooks:
+            self._start_stamps()   # before the first capture, so that every micro-batch has a record
         self._threads.append(thr)
         thr.start()
+
+    # ------------------------------------------------------------------ per-micro-batch timestamps
+    def add_send_timing_hook(self, hook: Callable[..., None], args: tuple) -> None:
+        """`hook(mbits, seconds, *args)` once per payload this stage sends to the next rank, from its device timestamps
+        (before or after `init()`; graphs captured without stamps are captured again). A stage without a next rank
+        (a world of one) sends nothing and never calls it, as on the Python-thread path."""
+        self._send_hooks.append((hook, args))
+        if self._pipe:
+            self._start_stamps()
+
+    def _start_stamps(self) -> None:
+        if self._drain_thread is not None:
+            return
+        check(LIB.pe_pipe_enable_stamps(self._pipe, 1))
+        pipe = self._pipe
+        self._drain = RecordDrain(lambda *a: LIB.pe_pipe_drain_stamps(pipe, *a), self._dispatch)
+        self._drain_thread = threading.Thread(target=self._drain_loop, daemon=True, name='pe-stamps')
+        self._drain_thread.start()
+
+    def _dispatch(self, rec: StampRecord) -> None:
+        calls = [(consumer, (rec,)) for consumer in self._record_cbs]
+        if self._rank_dst is not None:
+            calls += [(hook, (rec.send_mbits, rec.send_seconds, *args)) for hook, args in self._send_hooks]
+        for fn, args in calls:
+            try:
+                fn(*args)
+            except Exception:   # pylint: disable=broad-except
+                logger.exception("native pipeline: a timestamp record consumer failed")
+
+    def _drain_loop(self) -> None:
+        """Poll the ring (each C call releases the GIL and never waits on the device); a last pass after the stop."""
+        while True:
+            stopping = self._drain_stop.is_set()
+            got = self._drain.poll()
+            if stopping:
+                return
+            if got == 0:
+                self._drain_stop.wait(0.001)
+
+    @property
+    def records(self) -> int:
+        """Timestamp records dispatched so far (0 without stamps)."""
+        return self._drain.records if self._drain is not None else 0
+
+    @property
+    def records_dropped(self) -> int:
+        """Timestamp records overwritten before the drain thread read them."""
+        return self._drain.dropped if self._drain is not None else 0
 
     def _guard(self, fn) -> None:
         try:
@@ -328,6 +468,9 @@ class NativeStage:
             thr.join(timeout)
         if self._pipe:
             LIB.pe_pipe_sync(self._pipe)
+        if self._drain_thread is not None:
+            self._drain_stop.set()      # every graph has completed: the drain thread's last pass reads every record
+            self._drain_thread.join(timeout)
         if dist.is_initialized() and dist.get_world_size() > 1 and failure is None and self.exception is None:
             drain_barrier()   # no rank frees its ring while a neighbour's kernel may still store into it
         if self._pipe:

@@ -710,11 +710,32 @@ static PutPlan plan_put(int items, size_t n, int bit, bool aligned, int sms) {
   return pl;
 }
 
-int link_put(pe_link* l, const PutTensor* t, int n_tensors, int items, int bit, int clamp, cudaStream_t stream) {
+size_t link_payload_bytes(int items, size_t n, int bit, int wire_f16) {
+  if (bit == 0) return static_cast<size_t>(items) * n * (wire_f16 ? 2 : 4);
+  return static_cast<size_t>(items) * (quant_words(n, bit) * 4 + 2 * sizeof(float));
+}
+
+static bool put_aligned(const PutTensor& t) {
+  return (reinterpret_cast<uintptr_t>(t.a) & 15) == 0 && (t.b == nullptr || (reinterpret_cast<uintptr_t>(t.b) & 15) == 0);
+}
+
+int link_put(pe_link* l, const PutTensor* t, int n_tensors, int items, int bit, int clamp, cudaStream_t stream,
+             PutStamp* stamp) {
   PE_REQUIRE(l != nullptr && l->is_tx, "pe_link_put: not the producer end of a link");
   PE_REQUIRE(n_tensors >= 1 && n_tensors <= 2 && items > 0 && items <= kLinkMaxItems,
              "pe_link_put: %d tensors x %d items outside [1,2] x [1,%d]", n_tensors, items, kLinkMaxItems);
   PE_REQUIRE(bit >= 0 && bit <= 16, "pe_link_put: bit=%d outside [0,16]", bit);
+  int last_staged = -1;   // the tensor after whose encode kernels stamp->encoded is launched
+  if (stamp != nullptr) {
+    stamp->bytes = 0;
+    stamp->paths = 0;
+    for (int ti = 0; ti < n_tensors; ++ti) {
+      const int path = plan_put(items, t[ti].n, bit, put_aligned(t[ti]), sm_count()).path;
+      if (path == PE_LINK_PATH_STAGED) last_staged = ti;
+      stamp->paths |= 1 << path;
+      stamp->bytes += link_payload_bytes(items, t[ti].n, bit, l->wire_f16);
+    }
+  }
   size_t off = kLinkHeaderBytes;
   for (int ti = 0; ti < n_tensors; ++ti) {
     PE_REQUIRE(t[ti].a != nullptr && t[ti].n > 0, "pe_link_put: null / empty tensor %d", ti);
@@ -734,8 +755,7 @@ int link_put(pe_link* l, const PutTensor* t, int n_tensors, int items, int bit, 
     p.data_off = off;
     p.timeout_ns = l->timeout_ns;
     const size_t total = static_cast<size_t>(items) * t[ti].n;
-    const bool aligned = (reinterpret_cast<uintptr_t>(t[ti].a) & 15) == 0 &&
-                         (t[ti].b == nullptr || (reinterpret_cast<uintptr_t>(t[ti].b) & 15) == 0);
+    const bool aligned = put_aligned(t[ti]);
     const PutPlan pl = plan_put(items, t[ti].n, bit, aligned, sm_count());
     if (pl.path == PE_LINK_PATH_COPY) {
       PE_REQUIRE(aligned, "pe_link_put: payload tensors must be 16-byte aligned");
@@ -774,7 +794,8 @@ int link_put(pe_link* l, const PutTensor* t, int n_tensors, int items, int bit, 
       float* shift = reinterpret_cast<float*>(w + codes_bytes + roundup(items * sizeof(float), 256));
       float* alpha = reinterpret_cast<float*>(w + codes_bytes + 2 * roundup(items * sizeof(float), 256));
       void* work = w + codes_bytes + 2 * roundup(items * sizeof(float), 256) + 256;
-      const int rc = quant_encode_impl(x, items, t[ti].n, bit, clamp, codes, scale, shift, alpha, work, stream);
+      int rc = quant_encode_impl(x, items, t[ti].n, bit, clamp, codes, scale, shift, alpha, work, stream);
+      if (rc == PE_OK && ti == last_staged) rc = stamp->encoded(stamp->ctx, stream);
       if (rc != PE_OK) return rc;
       p.staged_codes = codes;
       p.staged_scale = scale;
@@ -1176,6 +1197,12 @@ int pe_debug_link_put_plan(int items, size_t n, int bit, int aligned, int* out5)
   out5[3] = static_cast<int>(pl.per);
   out5[4] = pl.cache;
   return PE_OK;
+}
+
+// Host-only: the payload bytes a put of one [items, n] tensor at `bit` bits writes (what a timestamped pipeline reports).
+size_t pe_link_payload_bytes(int items, size_t n, int bit, int wire_f16) {
+  if (items <= 0 || bit < 0 || bit > 16) return 0;
+  return pe::link_payload_bytes(items, n, bit, wire_f16);
 }
 
 }  // extern "C"

@@ -101,7 +101,21 @@ struct pe_link {
 
 namespace pe {
 
-int link_put(pe_link* link, const PutTensor* t, int n_tensors, int items, int bit, int clamp, cudaStream_t stream);
+// What a pipeline with timestamps (pipe.cu) asks of link_put: a launch between a staged put's stand-alone encode kernels
+// and its shipping kernel, and a description of what the put wrote.
+struct PutStamp {
+  int (*encoded)(void* ctx, cudaStream_t stream) = nullptr;   // after the encode kernels of the last staged tensor
+  void* ctx = nullptr;
+  size_t bytes = 0;   // out: payload bytes written (see link_payload_bytes), summed over the tensors
+  int paths = 0;      // out: OR of 1 << PE_LINK_PATH_* over the tensors
+};
+
+// Bytes a put of one [items, n] tensor at `bit` bits writes: the values (f32, or f16 with wire_f16), or the packed codes
+// plus the per-item scale and shift. Equal to what the Python-thread path moves for the same tensor when wire_f16 == 0.
+size_t link_payload_bytes(int items, size_t n, int bit, int wire_f16);
+
+int link_put(pe_link* link, const PutTensor* t, int n_tensors, int items, int bit, int clamp, cudaStream_t stream,
+             PutStamp* stamp = nullptr);
 // prewait: park in the one-warp wait kernel first (consumers that may wait long while other streams compute)
 int link_get(pe_link* link, void* dst0, void* dst1, int items, size_t n0, size_t n1, int n_tensors, cudaStream_t stream,
              bool prewait);

@@ -13,6 +13,8 @@
 // Replaces TensorWorkThread.run + the queue hand-offs of DistP2pPipelineStage (p2p/__init__.py:261-295,373-394,442-450):
 // FIFO per hop (tickets and flags are strictly ordered), back-pressure through the rings (a producer blocks - on the
 // device - until the consumer has released the slot; enqueue blocks on the host-fed ring).
+#include <string.h>
+
 #include <atomic>
 #include <map>
 #include <mutex>
@@ -27,6 +29,14 @@ void count_launches(int n);
 uint64_t launch_count_now();
 int require_sm90();
 constexpr int kPipeWindow = 8;   // graph launches the host may run ahead of the device
+static_assert(PE_PIPE_STAMP_DEPTH > kPipeWindow, "a record must outlive the launches the host may run ahead");
+
+// One record of the timestamp ring (mapped host memory). `seq` is written last: index + 1 once the record is complete,
+// 0 while its first stamp has started to overwrite it.
+struct StampSlot {
+  unsigned long long seq;
+  pe_pipe_record rec;
+};
 }  // namespace pe
 
 struct pe_pipe {
@@ -43,6 +53,7 @@ struct pe_pipe {
     int n_par = 0;                                      // parities captured so far
     int want_par = 1;                                   // 1 (send inside the main graph) or 2 (overlapped)
     int kernels = 0;
+    bool stamps = false;                                // captured with timestamp kernels
   };
   cudaEvent_t ev_main_done[2] = {nullptr, nullptr}, ev_put_done[2] = {nullptr, nullptr};
   bool put_pending[2] = {false, false};
@@ -68,16 +79,146 @@ struct pe_pipe {
   bool pending = false;
   long long pend[2] = {0, 0};
   long long out_dim = 0;   // > 0: outgoing tickets carry it instead of the incoming dim (last stage: result elements per item)
+  // per-micro-batch timestamps (pe_pipe_enable_stamps)
+  std::atomic<bool> stamps_on{false};
+  bool cap_stamps = false;                  // the capture in progress carries stamp kernels
+  pe::StampSlot* stamp_host = nullptr;      // the ring, PE_PIPE_STAMP_DEPTH records (cudaHostAllocMapped)
+  pe::StampSlot* stamp_dev = nullptr;       // ... its device alias
+  unsigned long long* stamp_ctr = nullptr;  // device: next record of the main graph [0] and of the send graph [1]
+  unsigned long long stamp_next = 0;        // drain: the next record to read
 };
 
 namespace pe {
 
-static bool find_graph(pe_pipe* p, int ubatch, long long dim1, pe_pipe::Graph* out) {
+// `current`: the graph must also have been captured with the stamps setting now in force (a graph captured the other way
+// counts as missing, so the next payload of its shape captures again)
+static bool find_graph(pe_pipe* p, int ubatch, long long dim1, pe_pipe::Graph* out, bool current = true) {
   std::lock_guard<std::mutex> lock(p->graphs_mu);
   auto it = p->graphs.find(std::make_pair(ubatch, dim1));
   if (it == p->graphs.end() || it->second.n_par < it->second.want_par) return false;   // every parity captured?
+  if (current && it->second.stamps != p->stamps_on.load()) return false;
   if (out != nullptr) *out = it->second;
   return true;
+}
+
+// ------------------------------------------------------------------------------------------------ timestamps
+// Which fields a stamp writes. A micro-batch's record gets, in order: Start (graph start, before the receive), Got
+// (receive done), Stage (the stage's last kernel done), SendStart, Encoded (staged sends only), SendEnd. With the send
+// inside the main graph, Stage and SendStart are one stamp; with an overlapped send, the send graph's stamps find the
+// record through their own counter, because send(i) runs while main(i + 1) already stamps record i + 1.
+enum : int {
+  kStampStart = 1, kStampGot = 2, kStampStage = 4, kStampSendStart = 8, kStampEncoded = 16, kStampSendEnd = 32,
+};
+
+struct StampArgs {
+  StampSlot* ring;                // device alias of the mapped host ring
+  unsigned long long* ctr;        // device counters: [0] main graph, [1] send graph
+  int ctr_idx;                    // the counter that names this stamp's record
+  int what;                       // kStamp* fields
+  int bump;                       // bit i: advance ctr[i] past this record
+  // kStampGot on a peer link: the receive's ring, whose slot header holds the payload's bit-width
+  const uint8_t* in_ring;
+  size_t in_slot_bytes;
+  int in_slots;
+  const uint64_t* in_seq;
+  // kStampSendEnd: the record's remaining fields
+  int items, bit_out, flags;
+  unsigned long long bytes_out;
+};
+
+// One thread: %globaltimer into the micro-batch's record. Launched WITHOUT programmatic dependent launch, so it starts
+// only after the kernel before it has completed; the PDL-launched stage kernel after it waits (griddepcontrol.wait) for
+// the stamp's completion, which is ordered after everything before the stamp.
+__global__ void __launch_bounds__(1) pipe_stamp_kernel(const StampArgs a) {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  const unsigned long long r = *reinterpret_cast<volatile unsigned long long*>(a.ctr + a.ctr_idx);
+  StampSlot* s = a.ring + r % PE_PIPE_STAMP_DEPTH;
+  volatile pe_pipe_record* rec = &s->rec;
+  if (a.what & kStampStart) {
+    *reinterpret_cast<volatile unsigned long long*>(&s->seq) = 0;   // a reader copying the old record sees it changed
+    __threadfence_system();
+    rec->t_start = t;
+    rec->t_encoded = 0;
+  }
+  if (a.what & kStampGot) {
+    rec->t_got = t;
+    int bit = -1;
+    if (a.in_ring != nullptr) {
+      // The slot of the payload just consumed. Its producer may already be rewriting that slot for a payload a whole
+      // ring later; the header's bit-width then changes only if the producer's own bit-width did in between.
+      const uint64_t seq = *reinterpret_cast<const volatile uint64_t*>(a.in_seq) - 1;
+      const LinkHeader* h = reinterpret_cast<const LinkHeader*>(a.in_ring + (seq % static_cast<uint64_t>(a.in_slots)) * a.in_slot_bytes);
+      bit = static_cast<int>(*reinterpret_cast<const volatile uint32_t*>(&h->t[0].bit));
+    }
+    rec->bit_in = bit;
+  }
+  if (a.what & kStampStage) rec->t_stage = t;
+  if (a.what & kStampSendStart) rec->t_send_start = t;
+  if (a.what & kStampEncoded) rec->t_encoded = t;
+  if (a.what & kStampSendEnd) {
+    rec->t_send_end = t;
+    rec->index = r;
+    rec->items = a.items;
+    rec->bit_out = a.bit_out;
+    rec->flags = a.flags;
+    rec->bytes_out = a.bytes_out;
+    __threadfence_system();   // every field of the record (earlier stamps fenced theirs) before the publication
+    asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(&s->seq), "l"(r + 1) : "memory");
+  } else {
+    __threadfence_system();
+  }
+  if (a.bump & 1) a.ctr[0] = r + 1;
+  if (a.bump & 2) a.ctr[1] = r + 1;
+}
+
+static int launch_stamp(pe_pipe* p, StampArgs a, cudaStream_t stream) {
+  a.ring = p->stamp_dev;
+  a.ctr = p->stamp_ctr;
+  pipe_stamp_kernel<<<1, 1, 0, stream>>>(a);
+  PE_CUDA(cudaGetLastError());
+  count_launches(1);
+  return PE_OK;
+}
+
+struct EncodedStamp {   // link_put's callback context on a staged send
+  pe_pipe* p;
+  int ctr_idx;
+};
+
+static int stamp_encoded(void* ctx, cudaStream_t stream) {
+  const EncodedStamp* e = static_cast<const EncodedStamp*>(ctx);
+  StampArgs a = {};
+  a.ctr_idx = e->ctr_idx;
+  a.what = kStampEncoded;
+  return launch_stamp(e->p, a, stream);
+}
+
+// The send of a capture with stamps: [SendStart] put [Encoded inside a staged put] SendEnd (publishes the record).
+static int put_stamped(pe_pipe* p, const PutTensor* t, int n_tensors, int items, int bit, int clamp, int overlap,
+                       cudaStream_t stream) {
+  const int ctr_idx = overlap != 0 ? 1 : 0;
+  StampArgs a = {};
+  a.ctr_idx = ctr_idx;
+  if (overlap != 0) {
+    a.what = kStampSendStart;
+    const int rc = launch_stamp(p, a, stream);
+    if (rc != PE_OK) return rc;
+  }
+  EncodedStamp ctx = {p, ctr_idx};
+  PutStamp ps;
+  ps.encoded = stamp_encoded;
+  ps.ctx = &ctx;
+  const int rc = link_put(p->out, t, n_tensors, items, bit, clamp, stream, &ps);
+  if (rc != PE_OK) return rc;
+  a.what = kStampSendEnd;
+  a.bump = overlap != 0 ? 2 : 3;
+  a.items = items;
+  a.bit_out = bit;
+  a.flags = (overlap != 0 ? PE_STAMP_OVERLAPPED : 0) | ((ps.paths & (1 << PE_LINK_PATH_FUSED)) ? PE_STAMP_FUSED : 0) |
+            ((ps.paths & (1 << PE_LINK_PATH_STAGED)) ? PE_STAMP_STAGED : 0);
+  a.bytes_out = ps.bytes;
+  return launch_stamp(p, a, stream);
 }
 
 static void destroy_graph(pe_pipe::Graph& g) {
@@ -91,7 +232,8 @@ static void destroy_graph(pe_pipe::Graph& g) {
 
 static int launch_graph(pe_pipe* p, int ubatch, long long dim1) {
   pe_pipe::Graph g;
-  PE_REQUIRE(find_graph(p, ubatch, dim1, &g), "pipe: no graph captured for micro-batch size %d / dim %lld", ubatch, dim1);
+  PE_REQUIRE(find_graph(p, ubatch, dim1, &g, false), "pipe: no graph captured for micro-batch size %d / dim %lld", ubatch,
+             dim1);
   const int w = static_cast<int>(p->launched % kPipeWindow);
   if (p->launched >= static_cast<uint64_t>(kPipeWindow)) PE_CUDA(cudaEventSynchronize(p->window[w]));
   if (p->timing_reset.exchange(0) != 0) {
@@ -194,6 +336,8 @@ int pe_pipe_destroy(pe_pipe* p) {
   if (p->ev_res_last != nullptr) cudaEventDestroy(p->ev_res_last);
   if (p->res_dev != nullptr) cudaFree(p->res_dev);
   if (p->res_host != nullptr) cudaFreeHost(p->res_host);
+  if (p->stamp_host != nullptr) cudaFreeHost(p->stamp_host);
+  if (p->stamp_ctr != nullptr) cudaFree(p->stamp_ctr);
   if (p->compute != nullptr) cudaStreamDestroy(p->compute);
   if (p->copy != nullptr) cudaStreamDestroy(p->copy);
   if (p->results != nullptr) cudaStreamDestroy(p->results);
@@ -221,14 +365,34 @@ int pe_pipe_capture_begin(pe_pipe* p, int ubatch, long long dim1, int parity, vo
   PE_CUDA(cudaStreamSynchronize(p->compute));
   PE_CUDA(cudaStreamSynchronize(p->put));
   p->cap_parity = parity;
+  p->cap_stamps = p->stamps_on.load();
+  if (parity == 1) {   // parity 1 follows its graph's parity 0, so that both replay the same kernels
+    std::lock_guard<std::mutex> lock(p->graphs_mu);
+    auto it = p->graphs.find(std::make_pair(ubatch, dim1));
+    if (it != p->graphs.end() && it->second.n_par == 1) p->cap_stamps = it->second.stamps;
+  }
   PE_CUDA(cudaStreamBeginCapture(p->compute, cudaStreamCaptureModeRelaxed));
   p->capturing = true;
   p->cap_ubatch = ubatch;
   p->cap_dim1 = dim1;
   p->cap_launch0 = launch_count_now();
-  int rc;
-  if (p->in->kind == 2) rc = link_get_raw(p->in, dst0, raw_bytes, p->compute, false);
-  else rc = link_get(p->in, dst0, dst1, ubatch, n0, n1, dst1 != nullptr ? 2 : 1, p->compute, false);
+  StampArgs st = {};
+  st.what = kStampStart;
+  int rc = p->cap_stamps ? launch_stamp(p, st, p->compute) : PE_OK;
+  if (rc == PE_OK) {
+    if (p->in->kind == 2) rc = link_get_raw(p->in, dst0, raw_bytes, p->compute, false);
+    else rc = link_get(p->in, dst0, dst1, ubatch, n0, n1, dst1 != nullptr ? 2 : 1, p->compute, false);
+  }
+  if (rc == PE_OK && p->cap_stamps) {
+    st.what = kStampGot;
+    if (p->in->kind != 2) {
+      st.in_ring = p->in->rx.ring;
+      st.in_slot_bytes = p->in->rx.slot_bytes;
+      st.in_slots = p->in->rx.n_slots;
+      st.in_seq = p->in->rx.seq;
+    }
+    rc = launch_stamp(p, st, p->compute);
+  }
   if (rc != PE_OK) pe_pipe_capture_abort(p);
   return rc;
 }
@@ -270,21 +434,31 @@ int pe_pipe_capture_end(pe_pipe* p, const void* a0, const void* b0, size_t n0, c
   PutTensor t[2] = {{static_cast<const float*>(a0), static_cast<const float*>(b0), n0},
                     {static_cast<const float*>(a1), static_cast<const float*>(b1), n1}};
   const int par = p->cap_parity;
+  const bool stamps = p->cap_stamps;
+  const int n_tensors = a1 != nullptr ? 2 : 1;
   cudaGraphExec_t exec_main = nullptr, exec_put = nullptr;
-  int rc;
-  if (overlap == 0) {
-    rc = link_put(p->out, t, a1 != nullptr ? 2 : 1, items, bit, clamp, p->compute);
-    if (rc != PE_OK) {
-      pe_pipe_capture_abort(p);
-      return rc;
-    }
+  int rc = PE_OK;
+  if (stamps) {   // the stage's last kernel is done (and, with the send in this graph, the send starts)
+    StampArgs st = {};
+    st.what = overlap != 0 ? kStampStage : (kStampStage | kStampSendStart);
+    st.bump = overlap != 0 ? 1 : 0;
+    rc = launch_stamp(p, st, p->compute);
+  }
+  if (rc == PE_OK && overlap == 0) {
+    rc = stamps ? put_stamped(p, t, n_tensors, items, bit, clamp, 0, p->compute)
+                : link_put(p->out, t, n_tensors, items, bit, clamp, p->compute);
+  }
+  if (rc != PE_OK) {
+    pe_pipe_capture_abort(p);
+    return rc;
   }
   p->capturing = false;
   rc = end_capture(p->compute, &exec_main, "cudaStreamEndCapture (pipe)");
   if (rc != PE_OK) return rc;
   if (overlap != 0) {
     PE_CUDA(cudaStreamBeginCapture(p->put, cudaStreamCaptureModeRelaxed));
-    rc = link_put(p->out, t, a1 != nullptr ? 2 : 1, items, bit, clamp, p->put);
+    rc = stamps ? put_stamped(p, t, n_tensors, items, bit, clamp, 1, p->put)
+                : link_put(p->out, t, n_tensors, items, bit, clamp, p->put);
     if (rc != PE_OK) {
       cudaGraph_t graph = nullptr;
       cudaStreamEndCapture(p->put, &graph);
@@ -310,6 +484,7 @@ int pe_pipe_capture_end(pe_pipe* p, const void* a0, const void* b0, size_t n0, c
     g.exec_put[par] = exec_put;
     g.n_par = par + 1;
     g.kernels = captured;
+    g.stamps = stamps;
     total = g.kernels;
   }
   if (kernels != nullptr) *kernels = total;
@@ -452,6 +627,67 @@ int pe_pipe_timing(pe_pipe* p, float* compute_ms, float* results_ms, unsigned lo
   }
   if (launches != nullptr) *launches = p->timed_launches;
   if (kernels != nullptr) *kernels = p->timed_kernels;
+  return PE_OK;
+}
+
+// Capture the next graphs with (on != 0) or without timestamp kernels. The ring is allocated on first use and kept.
+int pe_pipe_enable_stamps(pe_pipe* p, int on) {
+  using namespace pe;
+  PE_REQUIRE(p != nullptr, "pe_pipe_enable_stamps: null pipe");
+  if (on != 0 && p->stamp_host == nullptr) {
+    const size_t bytes = sizeof(StampSlot) * PE_PIPE_STAMP_DEPTH;
+    void* host = nullptr;
+    void* ctr = nullptr;
+    cudaError_t e = cudaHostAlloc(&host, bytes, cudaHostAllocMapped);
+    if (e == cudaSuccess) {
+      memset(host, 0, bytes);
+      e = cudaHostGetDevicePointer(reinterpret_cast<void**>(&p->stamp_dev), host, 0);
+    }
+    if (e == cudaSuccess) e = cudaMalloc(&ctr, 2 * sizeof(unsigned long long));
+    if (e == cudaSuccess) e = cudaMemset(ctr, 0, 2 * sizeof(unsigned long long));
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    if (e == cudaSuccess) {   // load the kernel's module now: inside a stream capture a first-use load could be refused
+      cudaFuncAttributes attr;
+      e = cudaFuncGetAttributes(&attr, pipe_stamp_kernel);
+    }
+    if (e != cudaSuccess) {
+      if (host != nullptr) cudaFreeHost(host);
+      if (ctr != nullptr) cudaFree(ctr);
+      p->stamp_dev = nullptr;
+      return check_cuda(e, "pe_pipe_enable_stamps");
+    }
+    p->stamp_ctr = static_cast<unsigned long long*>(ctr);
+    p->stamp_host = static_cast<StampSlot*>(host);
+  }
+  p->stamps_on.store(on != 0);
+  return PE_OK;
+}
+
+// A seqlock read of each record: its sequence word before and after the copy must both name it.
+int pe_pipe_drain_stamps(pe_pipe* p, pe_pipe_record* out, int max, int* n, unsigned long long* dropped) {
+  using namespace pe;
+  PE_REQUIRE(p != nullptr && (out != nullptr || max == 0) && max >= 0 && n != nullptr && dropped != nullptr,
+             "pe_pipe_drain_stamps: bad arguments");
+  *n = 0;
+  if (p->stamp_host == nullptr) return PE_OK;
+  constexpr unsigned long long kDepth = PE_PIPE_STAMP_DEPTH;
+  while (*n < max) {
+    const unsigned long long want = p->stamp_next + 1;
+    StampSlot* s = p->stamp_host + p->stamp_next % kDepth;
+    const unsigned long long s1 = __atomic_load_n(&s->seq, __ATOMIC_ACQUIRE);
+    if (s1 < want) break;   // not complete yet
+    if (s1 > want) {
+      // the slot already holds record s1 - 1 >= stamp_next + depth: every record older than s1 - depth is gone
+      *dropped += s1 - kDepth - p->stamp_next;
+      p->stamp_next = s1 - kDepth;
+      continue;
+    }
+    memcpy(&out[*n], &s->rec, sizeof(pe_pipe_record));
+    std::atomic_thread_fence(std::memory_order_acquire);
+    if (__atomic_load_n(&s->seq, __ATOMIC_RELAXED) == s1) ++*n;
+    else ++*dropped;   // overwritten while it was copied
+    ++p->stamp_next;
+  }
   return PE_OK;
 }
 

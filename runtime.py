@@ -62,8 +62,9 @@ MONITORING_KEY_RECV = 'recv'
 MONITORING_KEY_SEND = 'send'
 
 # Per-kernel-group heartbeats ('shard', 'quant_encode', 'quant_decode', 'output') cost four CUDA event records per
-# micro-batch and stage, so unlike the reference they are opt-in: MONITORING=1. The 'send' key is always fed when an
-# adaptive quantization policy is active.
+# micro-batch and stage on the Python-thread path, and timestamp kernels in every graph on the native pipeline, so
+# unlike the reference they are opt-in: MONITORING=1. The 'send' key is always fed when an adaptive quantization policy
+# is active.
 ENV_MONITORING: str = "MONITORING"
 _device_iters = None   # monitoring.DeviceIterations when MONITORING=1
 
@@ -71,6 +72,24 @@ _device_iters = None   # monitoring.DeviceIterations when MONITORING=1
 def monitoring_enabled() -> bool:
     """Whether the opt-in heartbeats are on."""
     return _device_iters is not None
+
+
+def enable_monitoring() -> None:
+    """Turn the opt-in heartbeats on (MONITORING=1): their keys in the `monitoring` context `monitoring.init` made."""
+    global _device_iters   # pylint: disable=global-statement
+    monitoring.add_key(MONITORING_KEY_MODEL, work_type='tensors', acc_type='layers')
+    monitoring.add_key(MONITORING_KEY_OUTPUT, work_type='classifications', acc_type='correct')
+    monitoring.add_key(MONITORING_KEY_QUANT_DECODE, work_type='tensors', acc_type='bits')
+    monitoring.add_key(MONITORING_KEY_QUANT_ENCODE, work_type='tensors', acc_type='bits')
+    _device_iters = monitoring.DeviceIterations()
+
+
+def disable_monitoring() -> None:
+    """Report the heartbeats still in flight and turn them off."""
+    global _device_iters   # pylint: disable=global-statement
+    if _device_iters is not None:
+        _device_iters.harvest(drain=True)
+        _device_iters = None
 
 
 def forward_pre_hook_monitor(_module, _inputs) -> None:
@@ -129,12 +148,59 @@ def forward_pre_hook_quant_decode(_module, input_arg: Tuple[Tuple[torch.Tensor, 
     return (tuple(forward_tensor),)         # a (data, skip) tuple payload
 
 
+def native_heartbeats(rec, n_layers: int, encode: bool, decode: bool) -> List[Tuple[str, float, int, int]]:
+    """The heartbeats `(key, seconds, work, accuracy)` the Python-thread path's hooks give for one micro-batch, from the
+    native pipeline's timestamp record of it (`_native.StampRecord`; device nanoseconds). `encode` / `decode`: the
+    stage has the quantisation hook of that side registered.
+
+    * shard: receive done -> the stage's last kernel done; work = items, accuracy = layers.
+    * quant_decode: on the native pipeline dequantisation is inside the receive kernel, so the key reports that
+      kernel's duration, measured from the graph's start - it includes the kernel's wait for the upstream payload.
+    * quant_encode: a staged send (generic bit-widths) reports its stand-alone encode kernels (send start -> encoded);
+      a fused send (2 / 4 / 8 / 16 bits) quantises inside the send kernel, so the key reports that whole kernel.
+    * An unquantised payload (bit 0) is not encoded or decoded: 0 s, like the thread path's pass-through hooks.
+    Both quantisation keys: work = items if bit > 0 else 0, accuracy = bit (`runtime.py:88-90,124-126`)."""
+    from pipeedge_b200._lib import PE_STAMP_STAGED   # pylint: disable=import-outside-toplevel
+    beats = [(MONITORING_KEY_MODEL, (rec.t_stage - rec.t_got) * 1e-9, rec.items, n_layers)]
+    if decode:
+        bit = rec.bit_in
+        beats.append((MONITORING_KEY_QUANT_DECODE, (rec.t_got - rec.t_start) * 1e-9 if bit > 0 else 0.0,
+                      rec.items if bit > 0 else 0, bit))
+    if encode:
+        bit = rec.bit_out
+        if bit == 0:
+            seconds = 0.0
+        elif rec.flags & PE_STAMP_STAGED:
+            seconds = (rec.t_encoded - rec.t_send_start) * 1e-9
+        else:
+            seconds = (rec.t_send_end - rec.t_send_start) * 1e-9
+        beats.append((MONITORING_KEY_QUANT_ENCODE, seconds, rec.items if bit > 0 else 0, bit))
+    return beats
+
+
+def _native_monitor_records(shard):
+    """With MONITORING=1, the native pipeline's per-micro-batch record consumer of `shard`: the heartbeats of
+    `native_heartbeats` for the hooks the shard carries. None (no timestamps) otherwise."""
+    if _device_iters is None:
+        return None
+    n_layers = shard.shard_config.layer_end - shard.shard_config.layer_start + 1
+    encode = forward_hook_quant_encode in shard._forward_hooks.values()            # pylint: disable=protected-access
+    decode = forward_pre_hook_quant_decode in shard._forward_pre_hooks.values()    # pylint: disable=protected-access
+
+    def consume(rec) -> None:
+        for key, seconds, work, accuracy in native_heartbeats(rec, n_layers, encode, decode):
+            monitoring.iteration(key, work=work, accuracy=accuracy, seconds=seconds)
+    return consume
+
+
 # What the native pipeline (pipeedge_b200/comm/p2p/_native.py) does with each hook: the quantisation pair is performed by
-# the links' send / receive kernels (same codes, same decoded values), the monitor pair is a no-op unless MONITORING=1.
+# the links' send / receive kernels (same codes, same decoded values); the monitor pair is fed from the graphs' device
+# timestamps when MONITORING=1 (`_pe_records`: the stage turns timestamps on and hands it every record).
 forward_hook_quant_encode._pe_native = True                 # pylint: disable=protected-access
 forward_pre_hook_quant_decode._pe_native = True             # pylint: disable=protected-access
-forward_pre_hook_monitor._pe_native = lambda: _device_iters is None    # pylint: disable=protected-access
-forward_hook_monitor._pe_native = lambda: _device_iters is None        # pylint: disable=protected-access
+forward_pre_hook_monitor._pe_native = True                  # pylint: disable=protected-access
+forward_hook_monitor._pe_native = True                      # pylint: disable=protected-access
+forward_hook_monitor._pe_records = _native_monitor_records  # pylint: disable=protected-access
 
 
 def _payload_tensors(outputs) -> Tuple[torch.Tensor, ...]:
@@ -414,15 +480,10 @@ def run_pipeline_p2p(world_size: int, rank: int, model_name: str, model_file: Op
                      rank_order: Optional[List[int]], data_rank: int, hosts: Optional[List[str]] = None,
                      sched_args: Optional[dict] = None) -> float:
     """Run the pipeline using P2P communication (`runtime.py:418-511`); returns throughput on the data rank."""
-    global _device_iters   # pylint: disable=global-statement
     throughput = 0.0
     monitoring.init(MONITORING_KEY_SEND, get_window_size(), work_type='Mbits')
     if os.getenv(ENV_MONITORING, '0') == '1':
-        monitoring.add_key(MONITORING_KEY_MODEL, work_type='tensors', acc_type='layers')
-        monitoring.add_key(MONITORING_KEY_OUTPUT, work_type='classifications', acc_type='correct')
-        monitoring.add_key(MONITORING_KEY_QUANT_DECODE, work_type='tensors', acc_type='bits')
-        monitoring.add_key(MONITORING_KEY_QUANT_ENCODE, work_type='tensors', acc_type='bits')
-        _device_iters = monitoring.DeviceIterations()
+        enable_monitoring()
     with DistP2pContext(('gloo',), {'world_size': world_size, 'rank': rank}, handle_cmd) as dist_ctx:
         if rank == 0:
             stage_layers, stage_quant, stage_ranks = get_pipeline_sched(world_size, partition, quant, rank_order,
@@ -470,6 +531,8 @@ def run_pipeline_p2p(world_size: int, rank: int, model_name: str, model_file: Op
             model.register_forward_pre_hook(devices.forward_pre_hook_to_device)
         with model_cfg.dist_p2p_pipeline_stage_factory(stage_ranks, data_rank, rank, stage, model,
                                                        handle_results) as stage_ctx:
+            if model is not None:
+                logger.info("Pipeline stage: %s", 'native' if stage_ctx.native is not None else 'Python threads')
             if os.getenv(ENV_ADAPTIVE_QUANT) or monitoring_enabled():
                 stage_ctx.register_send_timing_hook(hop_timing_hook_monitor, (MONITORING_KEY_SEND,))
             if rank == data_rank:
@@ -489,9 +552,7 @@ def run_pipeline_p2p(world_size: int, rank: int, model_name: str, model_file: Op
                 stop_event.set()
             else:
                 stop_event.wait()
-    if _device_iters is not None:
-        _device_iters.harvest(drain=True)
-        _device_iters = None
+    disable_monitoring()
     monitoring.finish()
     return throughput
 
