@@ -275,6 +275,15 @@ int pe_pipe_destroy(pe_pipe* pipe);
 void* pe_pipe_stream(pe_pipe* pipe);
 void* pe_pipe_copy_stream(pe_pipe* pipe);
 int pe_pipe_has_graph(pe_pipe* pipe, int ubatch, long long dim1);
+/* Graphs are filed per (ubatch, dim1, send bit-width): pe_pipe_capture_end's `bit`. The send bit-width set here picks the
+ * variant that pe_pipe_run / pe_pipe_submit launch and pe_pipe_has_graph reports, from the next launch on (an atomic
+ * store, legal while another thread runs the pipe). A bit-width without a graph for a payload's shape makes pe_pipe_run
+ * ask for a capture instead of launching another variant. -1, the initial value: each shape's most recent capture, and
+ * while it is in force a capture replaces the shape's graph of any other bit-width - a pipe that never calls this keeps
+ * and launches exactly what it did before. Set a bit-width before capturing to keep one graph per bit-width. */
+int pe_pipe_set_send_bit(pe_pipe* pipe, int bit);
+/* Whether the graph of (ubatch, dim1) for send bit-width `bit` is captured (with the stamps setting now in force). */
+int pe_pipe_has_variant(pe_pipe* pipe, int ubatch, long long dim1, int bit);
 /* Capture for buffer parity 0 (and, with an overlapped send, 1): begin enqueues the receive into dst0 / dst1, the caller
  * then enqueues the stage's kernels on pe_pipe_stream(), end adds the send - inside the same graph (overlap == 0) or as
  * a graph of its own on a second stream that overlaps the NEXT micro-batch's receive and first kernels (overlap != 0:

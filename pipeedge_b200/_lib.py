@@ -101,6 +101,8 @@ SYMBOLS = {
     'pe_pipe_stream': (c_void_p, [c_void_p]),
     'pe_pipe_copy_stream': (c_void_p, [c_void_p]),
     'pe_pipe_has_graph': (c_int, [c_void_p, c_int, c_longlong]),
+    'pe_pipe_set_send_bit': (c_int, [c_void_p, c_int]),
+    'pe_pipe_has_variant': (c_int, [c_void_p, c_int, c_longlong, c_int]),
     'pe_pipe_capture_begin': (c_int, [c_void_p, c_int, c_longlong, c_int, c_void_p, c_void_p, c_size_t, c_size_t, c_size_t]),
     'pe_pipe_capture_end': (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_size_t, c_int, c_int,
                                     c_int, c_int, POINTER(c_int)]),

@@ -16,6 +16,12 @@ once per (micro-batch size, sequence length): to capture the graph.
 Per-micro-batch timing: with stamps on (a shard hook that asks for records, or a send-timing hook), the graphs also
 write device timestamps into a ring of records in host memory (`pe_pipe_enable_stamps`); a drain thread turns each
 completed record into calls of the stage's record consumers and send-timing hooks, off the graph-launch path.
+
+Adaptive bit-widths: a shard hook may declare the bit-widths it sets `quant_bit` to (`_pe_send_bits`). A stage whose
+set S = {initial bit-width} | declared sets has more than one member captures one graph per bit-width in S for every
+shape, all at once, and picks the variant per micro-batch (`pe_pipe_set_send_bit`): after each record's consumers (a
+policy hook's record consumer decides the next bit-width there) and, on the data rank, at every `enqueue`. No kernel and
+no graph changes; switching never captures while payloads are in flight.
 """
 import collections
 import ctypes
@@ -23,7 +29,7 @@ import logging
 import os
 import threading
 import time
-from typing import Callable, List, NamedTuple, Optional
+from typing import Callable, Iterable, List, NamedTuple, Optional, Set, Tuple
 import torch
 import torch.distributed as dist
 from ... import _lib
@@ -58,6 +64,10 @@ def overlap_send() -> bool:
     return os.environ.get('PIPEEDGE_OVERLAP_SEND', '1') != '0'
 
 
+def _clamp(bit: int) -> int:
+    return _lib.PE_CLAMP_AUTO if bit > 0 else _lib.PE_CLAMP_NONE
+
+
 def hook_is_native(hook) -> bool:
     """Whether a module hook is represented by the native pipeline's kernels (quantisation encode / decode) or is a
     no-op there (device placement, disabled monitoring): marked by `_pe_native` (a bool or a callable)."""
@@ -87,6 +97,54 @@ def record_consumers(shard) -> List[Callable]:
         if consumer is not None:
             consumers.append(consumer)
     return consumers
+
+
+def declared_send_bits(shard) -> Set[int]:
+    """The bit-widths the shard's hooks may set its `quant_bit` to: the union of the hooks' `_pe_send_bits` (an iterable
+    of ints, or a callable returning one)."""
+    bits = set()
+    for hook in _shard_hooks(shard):
+        declared = getattr(hook, '_pe_send_bits', None)
+        if declared is not None:
+            bits.update(int(b) for b in (declared() if callable(declared) else declared))
+    return bits
+
+
+def wire_f16() -> bool:
+    """Whether links put raw payloads on the wire as fp16 (`PIPEEDGE_WIRE_F16=1`; read by the links at open)."""
+    return os.environ.get('PIPEEDGE_WIRE_F16', '0')[:1] == '1'
+
+
+def payload_fits(room: int, items: int, elems: Iterable[int], bit: int, wire: int) -> bool:
+    """Whether a payload of tensors [items, n] (n in `elems`) at `bit` bits fits `room` bytes of slot payload
+    (`pe_link_slot_bytes`), placed as `pe_link_put` places it: each tensor's wire bytes (the values, or the packed codes -
+    per-item scale and shift live in the slot header) at an offset rounded up to 256 bytes."""
+    off = 0
+    for n in elems:
+        wire_bytes = LIB.pe_link_payload_bytes(items, n, bit, wire) - (8 * items if bit > 0 else 0)
+        if off + wire_bytes > room:
+            return False
+        off += (wire_bytes + 255) // 256 * 256
+    return True
+
+
+class RecordShapeError(LookupError):
+    """A timestamp record matches no payload shape the stage has captured (or more than one)."""
+
+
+def record_payload_elems(rec, shapes: Iterable[Tuple[int, Tuple[int, ...]]]) -> Tuple[int, ...]:
+    """Elements per item of each tensor of the payload a record's micro-batch sent. `shapes`: (items, elements per item
+    of each tensor) of the payloads the stage has captured graphs for; the match is the one whose payload at the record's
+    bit-width has the record's size. It is unique: payloads of one item count differ by at least one row of the stage's
+    output (a BERT sequence length more or less), and every row adds bytes at every bit-width."""
+    wire = 1 if wire_f16() else 0
+    found = {elems for items, elems in shapes
+             if items == rec.items and sum(LIB.pe_link_payload_bytes(items, n, rec.bit_out, wire) for n in elems)
+             == rec.bytes_out}
+    if len(found) != 1:
+        raise RecordShapeError(f"native pipeline: {len(found)} captured payload shapes match the record of micro-batch "
+                          f"{rec.index} ({rec.items} items, {rec.bit_out} bits, {rec.bytes_out} bytes)")
+    return found.pop()
 
 
 class StampRecord(NamedTuple):
@@ -175,9 +233,17 @@ class NativeStage:
         self._capture_lock = threading.Lock()
         self.exception: Optional[BaseException] = None
         self.graph_kernels = {}               # (ubatch, dim1) -> kernels per micro-batch
+        self.variant_kernels = {}             # (ubatch, dim1, bit) -> kernels per micro-batch of that variant
+        self.captures = 0                     # graph variants captured so far (every parity of one counts once)
         self._result_shape = None
         self._captured_bit = None             # the QuantPipe bit-width the captured graphs send with
-        self._quant_key, self._quant_val = None, 0
+        self._quant_cache = (None, 0, 0)      # (quant_bit tensor, its in-place version, its value)
+        # Adaptive bit-widths: S = the initial bit-width | every set the shard's hooks declare; one graph per member
+        bit0 = self._quant()[0]
+        declared = set() if shard.shard_config.is_last else declared_send_bits(shard)
+        self._send_bits = sorted(declared | {bit0})
+        self.adaptive = len(self._send_bits) > 1
+        self._pushed_bit = None               # the last pe_pipe_set_send_bit (by one thread: enqueue's or the drain's)
         self._stream = None
         self._copy_stream = None
         self._record_cbs = record_consumers(shard)   # per-micro-batch record consumers (from the shard's hooks)
@@ -185,12 +251,15 @@ class NativeStage:
         self._drain = None                             # RecordDrain once stamps are on
         self._drain_stop = threading.Event()
         self._drain_thread = None
+        self._record_error: Optional[BaseException] = None   # a record no captured payload shape matched
 
     # ------------------------------------------------------------------ set-up
     def _open_link(self, sock, is_producer: bool, payload_bytes: int) -> ctypes.c_void_p:
         handle = ctypes.c_void_p()
+        # an adaptive producer announces a quantised payload even if it starts raw (it only sizes the receive grid)
+        hint = max(self._send_bits) if self.adaptive else self._quant()[0]
         check(LIB.pe_link_open(sock.fileno(), 1 if is_producer else 0, payload_bytes if is_producer else 0,
-                               link_slots() if is_producer else 0, self._quant()[0] if is_producer else 0,
+                               link_slots() if is_producer else 0, hint if is_producer else 0,
                                ctypes.byref(handle)))
         self._links.append(handle)
         return handle
@@ -237,6 +306,8 @@ class NativeStage:
         else:
             self._link_in, self._link_out = peer_in, peer_out
         check(LIB.pe_pipe_create(self._link_in, self._link_out, self._link_res, ctypes.byref(self._pipe)))
+        if self.adaptive:
+            self._push_bit()
         self._stream = torch.cuda.ExternalStream(LIB.pe_pipe_stream(self._pipe), device=self._device)
         self._copy_stream = torch.cuda.ExternalStream(LIB.pe_pipe_copy_stream(self._pipe), device=self._device)
         if shard.shard_config.is_last:
@@ -279,8 +350,25 @@ class NativeStage:
         for fn, args in calls:
             try:
                 fn(*args)
+            except RecordShapeError as exc:
+                # a consumer could not tell which micro-batch the record is (a policy would stop adapting): the stage
+                # fails at its owner's next check()
+                if self._record_error is None:
+                    self._record_error = exc
+                    logger.exception("native pipeline: a timestamp record matches no captured payload shape")
             except Exception:   # pylint: disable=broad-except
                 logger.exception("native pipeline: a timestamp record consumer failed")
+        if self.adaptive and not self._is_data:
+            # a policy among the consumers may have changed `quant_bit`: the stage loop launches that variant from its
+            # next micro-batch on. The data rank instead selects at every enqueue, on the thread that launches.
+            self._push_bit()
+
+    def _push_bit(self) -> None:
+        """The bit-width in `quant_bit` selects the graph variant from the next launch on."""
+        bit = self._quant()[0]
+        if bit != self._pushed_bit:
+            check(LIB.pe_pipe_set_send_bit(self._pipe, bit))
+            self._pushed_bit = bit
 
     def _drain_loop(self) -> None:
         """Poll the ring (each C call releases the GIL and never waits on the device); a last pass after the stop."""
@@ -319,19 +407,34 @@ class NativeStage:
         if shard.shard_config.is_last or not hasattr(shard, 'quant_bit'):
             return 0, _lib.PE_CLAMP_NONE
         qb = shard.quant_bit
-        key = (id(qb), getattr(qb, '_version', 0))
-        if key != self._quant_key:
-            self._quant_key, self._quant_val = key, int(qb)
-        bit = self._quant_val
-        return bit, (_lib.PE_CLAMP_AUTO if bit > 0 else _lib.PE_CLAMP_NONE)
+        version = getattr(qb, '_version', 0)
+        cached, cached_version, bit = self._quant_cache   # one tuple: the drain thread may call this concurrently
+        if qb is not cached or version != cached_version:
+            bit = int(qb)
+            self._quant_cache = (qb, version, bit)        # holds the tensor, so that its id cannot be reused
+        return bit, _clamp(bit)
+
+    @property
+    def send_bits(self) -> List[int]:
+        """The bit-widths this stage keeps a graph variant of per shape (one member: a fixed-bit stage)."""
+        return list(self._send_bits)
+
+    @property
+    def variants(self) -> int:
+        """Graph variants captured and held now, over every shape and bit-width."""
+        return len(self.variant_kernels)
 
     def invalidate(self) -> None:
         """Forget the captured graphs (they bake in the shard's `quant_bit` and buffer addresses): the next payload of
-        each shape captures again. For callers that change a stage's bit-width between micro-batches by hand - the
-        adaptive policies do it from forward hooks, which select the Python-thread path in the first place."""
+        each shape captures again. For callers that change a fixed-bit stage's bit-width between micro-batches by hand;
+        a stage whose hooks declare their bit-widths (`_pe_send_bits`) switches between captured variants instead."""
         with self._capture_lock:
-            check(LIB.pe_pipe_invalidate(self._pipe))
-            self.graph_kernels.clear()
+            self._invalidate_locked()
+
+    def _invalidate_locked(self) -> None:
+        check(LIB.pe_pipe_invalidate(self._pipe))
+        self.graph_kernels.clear()
+        self.variant_kernels.clear()
 
     def prepare(self, ubatch: int, dim1: int = 0) -> None:
         """Capture the graph for micro-batches of `ubatch` items (`dim1`: sequence length for BERT) ahead of the first
@@ -347,9 +450,14 @@ class NativeStage:
             if ubatch > max_ubatch():
                 raise ValueError(f"micro-batch of {ubatch} items exceeds PIPEEDGE_MAX_UBATCH={max_ubatch()}")
             if shard.native_needs_resize(ubatch, dim1) and self.graph_kernels:
-                check(LIB.pe_pipe_invalidate(self._pipe))   # the stage's workspace is about to be re-created
-                self.graph_kernels.clear()
-            bit, clamp = self._quant()
+                self._invalidate_locked()   # the stage's workspace is about to be re-created
+            bit = self._quant()[0]
+            if self.adaptive and bit not in self._send_bits:
+                self._send_bits = sorted(set(self._send_bits) | {bit})   # a bit-width no hook declared
+            # a fixed-bit stage: the one bit-width it sends with; an adaptive stage: every variant of this shape it does
+            # not hold yet, at once
+            bits = [b for b in self._send_bits if not LIB.pe_pipe_has_variant(self._pipe, ubatch, dim1, b)] \
+                if self.adaptive else [bit]
             overlap = overlap_send()
             with torch.cuda.stream(self._stream):
                 ins = self._inputs.get((ubatch, dim1))
@@ -357,31 +465,53 @@ class NativeStage:
                     ins = [torch.zeros(shape, dtype=dtype, device=torch.device('cuda', self._device))
                            for shape, dtype in shard.native_input_spec(ubatch, dim1)]
                     self._inputs[(ubatch, dim1)] = ins
-                kernels = ctypes.c_int(0)
-                for parity in range(2 if overlap else 1):
-                    # eager run on the same buffers first: sizes every persistent buffer and does all first-use work
-                    # (module loads, function attributes, tensor-map driver entry points) outside the capture
-                    shard.native_forward(ins, parity, defer=not overlap)
-                    self._stream.synchronize()
-                    if self._is_data:
-                        raw = ins[0].numel() * ins[0].element_size()
-                        check(LIB.pe_pipe_capture_begin(self._pipe, ubatch, dim1, parity, ins[0].data_ptr(), None, 0, 0, raw))
-                    else:
-                        n0 = ins[0].numel() // ubatch
-                        n1 = ins[1].numel() // ubatch if len(ins) > 1 else 0
-                        check(LIB.pe_pipe_capture_begin(self._pipe, ubatch, dim1, parity, ins[0].data_ptr(),
-                                                        ins[1].data_ptr() if len(ins) > 1 else None, n0, n1, 0))
-                    try:
-                        parts = shard.native_forward(ins, parity, defer=not overlap)
-                    except BaseException:
-                        LIB.pe_pipe_capture_abort(self._pipe)
-                        raise
-                    a0, b0, m0 = parts[0]
-                    a1, b1, m1 = parts[1] if len(parts) > 1 else (None, None, 0)
-                    check(LIB.pe_pipe_capture_end(self._pipe, a0, b0, m0, a1, b1, m1, ubatch, bit, clamp,
-                                                  1 if overlap else 0, ctypes.byref(kernels)))
-            self.graph_kernels[(ubatch, dim1)] = kernels.value
+                for variant_bit in bits:
+                    kernels = self._capture_variant(ins, ubatch, dim1, variant_bit, overlap,
+                                                    check_slots=self.adaptive and variant_bit == bits[0])
+                    self.variant_kernels[(ubatch, dim1, variant_bit)] = kernels
+                    self.captures += 1
+                    if variant_bit == bit:
+                        self.graph_kernels[(ubatch, dim1)] = kernels
             self._captured_bit = bit
+
+    def _check_slot_fits(self, parts, ubatch: int) -> None:
+        """Every bit-width of an adaptive stage's set fits the downstream link's slots (sized for the raw payload)."""
+        room = LIB.pe_link_slot_bytes(self._link_out)
+        elems = [m for _, _, m in parts]
+        for bit in self._send_bits:
+            if not payload_fits(room, ubatch, elems, bit, 1 if wire_f16() else 0):
+                raise ValueError(f"native pipeline: a {bit}-bit payload of {ubatch} items x {elems} elements does not "
+                                 f"fit the link's {room}-byte slots (bit-widths of this stage: {self._send_bits})")
+
+    def _capture_variant(self, ins, ubatch: int, dim1: int, bit: int, overlap: bool, check_slots: bool) -> int:
+        """Capture the graph(s) of one (shape, send bit-width): both buffer parities with an overlapped send."""
+        shard = self._shard
+        kernels = ctypes.c_int(0)
+        for parity in range(2 if overlap else 1):
+            # eager run on the same buffers first: sizes every persistent buffer and does all first-use work
+            # (module loads, function attributes, tensor-map driver entry points) outside the capture
+            parts = shard.native_forward(ins, parity, defer=not overlap)
+            self._stream.synchronize()
+            if check_slots and parity == 0:
+                self._check_slot_fits(parts, ubatch)
+            if self._is_data:
+                raw = ins[0].numel() * ins[0].element_size()
+                check(LIB.pe_pipe_capture_begin(self._pipe, ubatch, dim1, parity, ins[0].data_ptr(), None, 0, 0, raw))
+            else:
+                n0 = ins[0].numel() // ubatch
+                n1 = ins[1].numel() // ubatch if len(ins) > 1 else 0
+                check(LIB.pe_pipe_capture_begin(self._pipe, ubatch, dim1, parity, ins[0].data_ptr(),
+                                                ins[1].data_ptr() if len(ins) > 1 else None, n0, n1, 0))
+            try:
+                parts = shard.native_forward(ins, parity, defer=not overlap)
+            except BaseException:
+                LIB.pe_pipe_capture_abort(self._pipe)
+                raise
+            a0, b0, m0 = parts[0]
+            a1, b1, m1 = parts[1] if len(parts) > 1 else (None, None, 0)
+            check(LIB.pe_pipe_capture_end(self._pipe, a0, b0, m0, a1, b1, m1, ubatch, bit, _clamp(bit),
+                                          1 if overlap else 0, ctypes.byref(kernels)))
+        return kernels.value
 
     # ------------------------------------------------------------------ data rank
     def enqueue(self, tensor: torch.Tensor) -> None:
@@ -390,7 +520,12 @@ class NativeStage:
         shape, dtype = self._shard.native_input_spec(tensor.shape[0], 0)[0]
         dim1 = int(tensor.shape[1]) if len(shape) == 2 else 0          # BERT: the sequence length is the payload's
         ubatch = int(tensor.shape[0])
-        if self._captured_bit is not None and self._quant()[0] != self._captured_bit:
+        bit = self._quant()[0]
+        if self.adaptive:
+            if bit not in self._send_bits:
+                self.invalidate()     # a bit-width outside the declared set: captured again, with the set
+            self._push_bit()
+        elif self._captured_bit is not None and bit != self._captured_bit:
             self.invalidate()     # the data rank's own bit-width was changed since its graphs were captured
         if not LIB.pe_pipe_has_graph(self._pipe, ubatch, dim1):
             self._capture(ubatch, dim1)
@@ -437,6 +572,9 @@ class NativeStage:
         """Re-raise what killed a native thread."""
         if self.exception is not None:
             raise RuntimeError("a native pipeline thread failed") from self.exception
+        if self._record_error is not None:
+            raise RuntimeError("a timestamp record of the native pipeline matched no captured payload shape") \
+                from self._record_error
 
     def timing_reset(self) -> None:
         """The next micro-batch starts a new device-timed phase."""

@@ -2,9 +2,9 @@
 //
 // A stage's whole micro-batch - link get (wait for the upstream payload, copy / dequantise it into the stage's fixed
 // input buffer) -> embeddings / encoder blocks / head kernels -> link put (quantise-and-send into the downstream ring) -
-// is captured ONCE per (micro-batch size, sequence length) into a CUDA graph: the link kernels find their ring slot
-// through device-resident sequence counters (link.cu), so the graph takes no per-payload arguments and the first
-// replay is already the steady state. The host side of a stage is this loop:
+// is captured ONCE per (micro-batch size, sequence length, send bit-width) into a CUDA graph: the link kernels find
+// their ring slot through device-resident sequence counters (link.cu), so the graph takes no per-payload arguments and
+// the first replay is already the steady state. The host side of a stage is this loop:
 //     read a 16-byte ticket from the upstream hop's socket (blocks) -> cudaGraphLaunch -> write the ticket downstream
 // i.e. two system calls and one launch per micro-batch; ordering against the neighbours' GPUs is entirely on the
 // devices (flags in peer memory). The data rank feeds its first stage through a host-fed link (pe_pipe_submit: H2D /
@@ -13,11 +13,13 @@
 // Replaces TensorWorkThread.run + the queue hand-offs of DistP2pPipelineStage (p2p/__init__.py:261-295,373-394,442-450):
 // FIFO per hop (tickets and flags are strictly ordered), back-pressure through the rings (a producer blocks - on the
 // device - until the consumer has released the slot; enqueue blocks on the host-fed ring).
+#include <limits.h>
 #include <string.h>
 
 #include <atomic>
 #include <map>
 #include <mutex>
+#include <tuple>
 #include <utility>
 
 #include "../../include/pipeedge_b200.h"
@@ -58,7 +60,12 @@ struct pe_pipe {
   cudaEvent_t ev_main_done[2] = {nullptr, nullptr}, ev_put_done[2] = {nullptr, nullptr};
   bool put_pending[2] = {false, false};
   int cap_parity = 0;
-  std::map<std::pair<int, long long>, Graph> graphs;
+  // (micro-batch size, dim1, send bit-width) -> graph. A stage whose bit-width changes between micro-batches keeps one
+  // graph per bit-width and picks one per launch (send_bit); the kernels and graphs of each variant are those of a
+  // fixed-bit stage at that bit-width.
+  std::map<std::tuple<int, long long, int>, Graph> graphs;
+  std::map<std::pair<int, long long>, int> latest_bit;   // bit-width of each shape's most recent capture
+  std::atomic<int> send_bit{-1};   // pe_pipe_set_send_bit; -1: the shape's most recent capture, whatever its bit-width
   std::mutex graphs_mu;    // prepare() on the owner thread may insert while the stage thread looks a graph up
   bool capturing = false;
   int cap_ubatch = 0;
@@ -90,11 +97,17 @@ struct pe_pipe {
 
 namespace pe {
 
-// `current`: the graph must also have been captured with the stamps setting now in force (a graph captured the other way
-// counts as missing, so the next payload of its shape captures again)
-static bool find_graph(pe_pipe* p, int ubatch, long long dim1, pe_pipe::Graph* out, bool current = true) {
+// `bit`: the send bit-width of the variant (-1: the shape's most recent capture). `current`: the graph must also have been
+// captured with the stamps setting now in force (a graph captured the other way counts as missing, so the next payload
+// of its shape captures again)
+static bool find_graph(pe_pipe* p, int ubatch, long long dim1, int bit, pe_pipe::Graph* out, bool current = true) {
   std::lock_guard<std::mutex> lock(p->graphs_mu);
-  auto it = p->graphs.find(std::make_pair(ubatch, dim1));
+  if (bit < 0) {
+    auto lb = p->latest_bit.find(std::make_pair(ubatch, dim1));
+    if (lb == p->latest_bit.end()) return false;
+    bit = lb->second;
+  }
+  auto it = p->graphs.find(std::make_tuple(ubatch, dim1, bit));
   if (it == p->graphs.end() || it->second.n_par < it->second.want_par) return false;   // every parity captured?
   if (current && it->second.stamps != p->stamps_on.load()) return false;
   if (out != nullptr) *out = it->second;
@@ -230,10 +243,10 @@ static void destroy_graph(pe_pipe::Graph& g) {
   g.n_par = 0;
 }
 
-static int launch_graph(pe_pipe* p, int ubatch, long long dim1) {
+static int launch_graph(pe_pipe* p, int ubatch, long long dim1, int bit) {
   pe_pipe::Graph g;
-  PE_REQUIRE(find_graph(p, ubatch, dim1, &g, false), "pipe: no graph captured for micro-batch size %d / dim %lld", ubatch,
-             dim1);
+  PE_REQUIRE(find_graph(p, ubatch, dim1, bit, &g, false),
+             "pipe: no graph captured for micro-batch size %d / dim %lld / send bit-width %d", ubatch, dim1, bit);
   const int w = static_cast<int>(p->launched % kPipeWindow);
   if (p->launched >= static_cast<uint64_t>(kPipeWindow)) PE_CUDA(cudaEventSynchronize(p->window[w]));
   if (p->timing_reset.exchange(0) != 0) {
@@ -350,8 +363,24 @@ int pe_pipe_destroy(pe_pipe* p) {
 void* pe_pipe_stream(pe_pipe* p) { return p == nullptr ? nullptr : p->compute; }
 void* pe_pipe_copy_stream(pe_pipe* p) { return p == nullptr ? nullptr : p->copy; }
 
+// For the send bit-width now in force (pe_pipe_set_send_bit).
 int pe_pipe_has_graph(pe_pipe* p, int ubatch, long long dim1) {
-  return (p != nullptr && pe::find_graph(p, ubatch, dim1, nullptr)) ? 1 : 0;
+  return (p != nullptr && pe::find_graph(p, ubatch, dim1, p->send_bit.load(), nullptr)) ? 1 : 0;
+}
+
+// For one send bit-width, whichever is in force (-1: the shape's most recent capture).
+int pe_pipe_has_variant(pe_pipe* p, int ubatch, long long dim1, int bit) {
+  return (p != nullptr && pe::find_graph(p, ubatch, dim1, bit, nullptr)) ? 1 : 0;
+}
+
+// The send bit-width whose graphs launch from the next launch on (-1, the initial value: each shape's most recent
+// capture). An atomic store: legal while another thread sits in pe_pipe_run or pe_pipe_submit, which read it once per
+// micro-batch. A bit-width without a graph for a payload's shape makes pe_pipe_run ask for a capture (and
+// pe_pipe_submit fail) rather than launch another variant.
+int pe_pipe_set_send_bit(pe_pipe* p, int bit) {
+  PE_REQUIRE(p != nullptr && bit >= -1 && bit <= 16, "pe_pipe_set_send_bit: bit=%d outside [-1,16]", bit);
+  p->send_bit.store(bit);
+  return PE_OK;
 }
 
 // Start capturing the graph for micro-batches of `ubatch` items (`dim1`: sequence length, part of the key). The get
@@ -366,9 +395,10 @@ int pe_pipe_capture_begin(pe_pipe* p, int ubatch, long long dim1, int parity, vo
   PE_CUDA(cudaStreamSynchronize(p->put));
   p->cap_parity = parity;
   p->cap_stamps = p->stamps_on.load();
-  if (parity == 1) {   // parity 1 follows its graph's parity 0, so that both replay the same kernels
+  if (parity == 1) {   // parity 1 follows its graph's parity 0 (the shape's latest capture): both replay the same kernels
     std::lock_guard<std::mutex> lock(p->graphs_mu);
-    auto it = p->graphs.find(std::make_pair(ubatch, dim1));
+    auto lb = p->latest_bit.find(std::make_pair(ubatch, dim1));
+    auto it = lb == p->latest_bit.end() ? p->graphs.end() : p->graphs.find(std::make_tuple(ubatch, dim1, lb->second));
     if (it != p->graphs.end() && it->second.n_par == 1) p->cap_stamps = it->second.stamps;
   }
   PE_CUDA(cudaStreamBeginCapture(p->compute, cudaStreamCaptureModeRelaxed));
@@ -425,12 +455,26 @@ static int end_capture(cudaStream_t stream, cudaGraphExec_t* exec, const char* w
 // Finish the capture started by pe_pipe_capture_begin for its parity: the put of the stage's output (x_i = a_i + b_i when
 // b_i != NULL; QuantPipe `bit` / `clamp` as pe_link_put) goes into the same graph (overlap == 0; parity must be 0) or
 // into a graph of its own on the send stream (overlap != 0: capture parity 0 AND 1, each over its own output buffers).
+// The graph is filed under (ubatch, dim1, bit); parity 1 completes the parity 0 capture of the same bit-width.
 // *kernels = kernels per micro-batch.
 int pe_pipe_capture_end(pe_pipe* p, const void* a0, const void* b0, size_t n0, const void* a1, const void* b1, size_t n1,
                         int items, int bit, int clamp, int overlap, int* kernels) {
   using namespace pe;
   PE_REQUIRE(p != nullptr && p->capturing, "pe_pipe_capture_end: no capture in progress");
   PE_REQUIRE(overlap != 0 || p->cap_parity == 0, "pe_pipe_capture_end: parity 1 exists only with an overlapped send");
+  if (p->cap_parity == 1) {
+    bool has_par0 = false;
+    {
+      std::lock_guard<std::mutex> lock(p->graphs_mu);
+      auto it = p->graphs.find(std::make_tuple(p->cap_ubatch, p->cap_dim1, bit));
+      has_par0 = it != p->graphs.end() && it->second.n_par == 1;
+    }
+    if (!has_par0) {
+      pe_pipe_capture_abort(p);
+      set_error("pe_pipe_capture_end: parity 1 of bit-width %d without its parity 0", bit);
+      return PE_ERR_INVALID;
+    }
+  }
   PutTensor t[2] = {{static_cast<const float*>(a0), static_cast<const float*>(b0), n0},
                     {static_cast<const float*>(a1), static_cast<const float*>(b1), n1}};
   const int par = p->cap_parity;
@@ -477,8 +521,23 @@ int pe_pipe_capture_end(pe_pipe* p, const void* a0, const void* b0, size_t n0, c
   int total = captured;
   {
     std::lock_guard<std::mutex> lock(p->graphs_mu);
-    pe_pipe::Graph& g = p->graphs[std::make_pair(p->cap_ubatch, p->cap_dim1)];
-    if (par == 0) destroy_graph(g);   // a fresh capture of this key starts with parity 0
+    pe_pipe::Graph& g = p->graphs[std::make_tuple(p->cap_ubatch, p->cap_dim1, bit)];
+    if (par == 0) {   // a fresh capture of this key starts with parity 0
+      destroy_graph(g);
+      p->latest_bit[std::make_pair(p->cap_ubatch, p->cap_dim1)] = bit;
+      if (p->send_bit.load() < 0) {
+        // no bit-width selected: the capture replaces the shape's graph, whatever bit-width that one sent with
+        for (auto it = p->graphs.lower_bound(std::make_tuple(p->cap_ubatch, p->cap_dim1, INT_MIN));
+             it != p->graphs.end() && std::get<0>(it->first) == p->cap_ubatch && std::get<1>(it->first) == p->cap_dim1;) {
+          if (std::get<2>(it->first) == bit) {
+            ++it;
+            continue;
+          }
+          destroy_graph(it->second);
+          it = p->graphs.erase(it);
+        }
+      }
+    }
     g.want_par = overlap != 0 ? 2 : 1;
     g.exec[par] = exec_main;
     g.exec_put[par] = exec_put;
@@ -499,6 +558,7 @@ int pe_pipe_invalidate(pe_pipe* p) {
   std::lock_guard<std::mutex> lock(p->graphs_mu);
   for (auto& kv : p->graphs) pe::destroy_graph(kv.second);
   p->graphs.clear();
+  p->latest_bit.clear();
   return PE_OK;
 }
 
@@ -507,9 +567,13 @@ int pe_pipe_invalidate(pe_pipe* p) {
 int pe_pipe_submit(pe_pipe* p, const void* src, size_t bytes, int src_is_host, int ubatch, long long dim1) {
   using namespace pe;
   PE_REQUIRE(p != nullptr && p->in->kind == 2, "pe_pipe_submit: this pipe's input is not host-fed");
+  const int bit = p->send_bit.load();
+  // refused before the input is fed: a micro-batch without its graph must not occupy the input ring
+  PE_REQUIRE(find_graph(p, ubatch, dim1, bit, nullptr, false),
+             "pipe: no graph captured for micro-batch size %d / dim %lld / send bit-width %d", ubatch, dim1, bit);
   int rc = link_feed(p->in, src, bytes, src_is_host, p->copy);
   if (rc != PE_OK) return rc;
-  rc = launch_graph(p, ubatch, dim1);
+  rc = launch_graph(p, ubatch, dim1, bit);
   if (rc != PE_OK) return rc;
   return link_ticket_send(p->out, ubatch, p->out_dim > 0 ? p->out_dim : dim1);
 }
@@ -547,14 +611,15 @@ int pe_pipe_run(pe_pipe* p, long long* need2) {
       }
     }
     const int ubatch = static_cast<int>(p->pend[0]);
-    if (!find_graph(p, ubatch, p->pend[1], nullptr)) {
+    const int bit = p->send_bit.load();   // one read per micro-batch: the check and the launch agree
+    if (!find_graph(p, ubatch, p->pend[1], bit, nullptr)) {
       p->pending = true;
       need2[0] = p->pend[0];
       need2[1] = p->pend[1];
       return 2;
     }
     p->pending = false;
-    int rc = launch_graph(p, ubatch, p->pend[1]);
+    int rc = launch_graph(p, ubatch, p->pend[1], bit);
     if (rc != PE_OK) return rc;
     rc = link_ticket_send(p->out, p->pend[0], p->out_dim > 0 ? p->out_dim : p->pend[1]);
     if (rc != PE_OK) return rc;

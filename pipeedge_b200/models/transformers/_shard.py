@@ -198,6 +198,12 @@ class GpuTransformerShard(ModuleShard):
         widths = {0: 2 * stage.hidden, 2: stage.inter + stage.hidden}.get(stage.last_sub, stage.hidden)
         return max_ubatch * max_tokens * widths * 4 + 8192
 
+    def native_payload_shapes(self):
+        """{(items, (elements per item of each output tensor))} for every input shape `native_forward` has run: the
+        payloads the stage's graphs send (the record consumers of the native pipeline map a record back to one)."""
+        keep = list(getattr(self, '_native_keep', {}).values())   # one C-level copy: a capture may add to it meanwhile
+        return {(outs[0].shape[0], tuple(t.numel() // outs[0].shape[0] for t in outs)) for outs in keep}
+
     def native_max_tokens(self) -> int:
         """Largest sequence length a payload can have."""
         return self.stage.tokens

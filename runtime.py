@@ -7,7 +7,8 @@ same hook structure around the shard (`run_pipeline_p2p`, `runtime.py:418-511`).
 activations stay in HBM, the hop is NCCL on a side stream, and the QuantPipe hooks call the fused device
 kernels (bit-identical codes). The adaptive QuantPipe policies (`ADAPTIVE_QUANT=HEURISTIC|HEURISTIC2|CONTROLLER`
 with `SEND_CONSTRAINT` items/s and `WINDOW_SIZE`, `runtime.py:121-216`) are carried over; they read the hop's
-DEVICE-side transfer time (CUDA events around the NCCL sends) through `monitoring.py`'s window statistics.
+DEVICE-side transfer time (CUDA events around the NCCL sends, or the native pipeline's graph timestamps) through
+`monitoring.py`'s window statistics.
 Scheduler-generated partitions are ingested in the scheduler's own YAML format (`parse_yaml_sched`, `-H`, `--sched-file`, or
 the reference's `sched-pipeline` binary when it is on PATH with `-sm/-sdt/-sd`). What is NOT carried over (out of scope,
 SURVEY.md section 2): the RPC backend (`-c rpc`), the `sched-pipeline` planner itself, energy monitoring, and the dataset loaders that need the network; inputs are the reference's synthetic fallback (`runtime.py:386-400`)
@@ -216,6 +217,11 @@ def _send_window(*getters: str):
     return (tag, window_size) + values
 
 
+# (largest compression ratio, bit-width) steps of the heuristic; beyond the last step it sends with the floor
+_HEURISTIC_STEPS = ((1, 0), (2, 16), (4, 8), (5, 6), (8, 4))
+_HEURISTIC_FLOOR = 2
+
+
 def forward_hook_set_quant_bandwidth_heuristic(module, _inputs, outputs) -> None:
     """Pick the quantization bit-width whose compression fits the window's send budget (`runtime.py:121-154`).
 
@@ -234,13 +240,16 @@ def forward_hook_set_quant_bandwidth_heuristic(module, _inputs, outputs) -> None
     quant_bit = module.quant_bit.item()
     unquantized_mbits = sent_mbits * (32 / quant_bit) if quant_bit > 0 else sent_mbits
     compress_ratio = int(unquantized_mbits / budget_mbits) + 1
-    for limit, bits in ((1, 0), (2, 16), (4, 8), (5, 6), (8, 4)):
+    for limit, bits in _HEURISTIC_STEPS:
         if compress_ratio <= limit:
             module.quant_bit = torch.tensor(bits)
             break
     else:
-        module.quant_bit = torch.tensor(2)
+        module.quant_bit = torch.tensor(_HEURISTIC_FLOOR)
     logger.info("Adaptive quantization (heuristic): bitwidth=%d", int(module.quant_bit))
+
+
+_HEURISTIC2_MIN_BIT = 2
 
 
 def forward_hook_set_quant_bandwidth_heuristic_2(module, _inputs, outputs) -> None:
@@ -255,7 +264,7 @@ def forward_hook_set_quant_bandwidth_heuristic_2(module, _inputs, outputs) -> No
     src_bit = torch.tensor(tensors[0].element_size() * 8)
     quant_bit = quantutil.constrain_max_bitwidth(ubatch_time, ubatch_mbits, bandwidth, src_bit)
     # at least 2 bits; the source width itself means "do not quantize" (0)
-    module.quant_bit = max(torch.tensor(2), quant_bit) % src_bit
+    module.quant_bit = max(torch.tensor(_HEURISTIC2_MIN_BIT), quant_bit) % src_bit
     logger.info("Adaptive quantization (heuristic2): bitwidth=%d", int(module.quant_bit))
 
 
@@ -291,6 +300,41 @@ def forward_hook_set_quant_controller(module, _inputs, outputs) -> None:
     bitwidth = bw1 if bw1_iters > 0 else bw2
     module.quant_bit = torch.tensor(bitwidth % max(BITWIDTHS))               # the widest setting = no quantization
     module.register_buffer('bitwidth1_iters', torch.tensor(max(0, bw1_iters - 1)), persistent=False)
+
+
+def _native_policy_records(hook):
+    """The native pipeline's record consumer factory for a policy hook (`_pe_records`): the consumer calls the same hook
+    once per record of the stage, with a stand-in `outputs` of that micro-batch's geometry (meta fp32 tensors of
+    [items, elements per item] per payload tensor, recovered from the record and the shapes the stage captured). The
+    decision applies to the stage's next graph launch instead of the micro-batch the hook ran for."""
+    def factory(shard):
+        from pipeedge_b200.comm.p2p import _native   # pylint: disable=import-outside-toplevel
+
+        def consume(rec) -> None:
+            elems = _native.record_payload_elems(rec, shard.native_payload_shapes())
+            outputs = tuple(torch.empty((rec.items, n), dtype=torch.float32, device='meta') for n in elems)
+            hook(shard, None, outputs[0] if len(outputs) == 1 else outputs)
+        return consume
+    return factory
+
+
+# The bit-widths each policy sets `quant_bit` to (the native pipeline captures one graph per member, `_pe_send_bits`).
+# HEURISTIC: its steps and floor. HEURISTIC2: `max(_HEURISTIC2_MIN_BIT, b) % src_bit` of every b that
+# `constrain_max_bitwidth` can return for an fp32 payload (src_bit 32, the native pipeline's payloads): src_bit itself,
+# 0, and the largest bit-width of each packing ratio below src_bit. CONTROLLER: BITWIDTHS with the widest as 0.
+_FP32_BITS = 32
+QUANT_BITS_HEURISTIC = frozenset(b for _, b in _HEURISTIC_STEPS) | {_HEURISTIC_FLOOR}
+QUANT_BITS_HEURISTIC2 = frozenset(max(_HEURISTIC2_MIN_BIT, b) % _FP32_BITS for b in range(_FP32_BITS, -1, -1)
+                                  if b in (0, _FP32_BITS) or int(compression_factor(b)) > int(compression_factor(b + 1)))
+QUANT_BITS_CONTROLLER = frozenset(b % max(BITWIDTHS) for b in BITWIDTHS)
+
+for _hook, _bits in ((forward_hook_set_quant_bandwidth_heuristic, QUANT_BITS_HEURISTIC),
+                     (forward_hook_set_quant_bandwidth_heuristic_2, QUANT_BITS_HEURISTIC2),
+                     (forward_hook_set_quant_controller, QUANT_BITS_CONTROLLER)):
+    _hook._pe_native = True                          # pylint: disable=protected-access
+    _hook._pe_records = _native_policy_records(_hook)   # pylint: disable=protected-access
+    _hook._pe_send_bits = _bits                      # pylint: disable=protected-access
+del _hook, _bits
 
 
 def hop_timing_hook_monitor(mbits: float, seconds: float, key: str) -> None:
