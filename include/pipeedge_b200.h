@@ -288,8 +288,16 @@ int pe_pipe_has_variant(pe_pipe* pipe, int ubatch, long long dim1, int bit);
  * then enqueues the stage's kernels on pe_pipe_stream(), end adds the send - inside the same graph (overlap == 0) or as
  * a graph of its own on a second stream that overlaps the NEXT micro-batch's receive and first kernels (overlap != 0:
  * the stage must write its output into a different buffer set per parity; micro-batch i uses parity i mod 2). */
+/* raw_bytes > 0 on a hop input: the first stage fed by a data rank outside the stage pipeline - the relayed input
+ * (pe_pipe_capture_relay) lands unchanged in dst0, after its header was checked against raw_bytes and ubatch. */
 int pe_pipe_capture_begin(pe_pipe* pipe, int ubatch, long long dim1, int parity, void* dst0, void* dst1, size_t n0,
                           size_t n1, size_t raw_bytes);
+/* Data rank outside the stage pipeline (pe_pipe_create(host-fed link, producer end of the hop to the first stage,
+ * consumer end of the hop from the last stage)): capture the graph that relays each input micro-batch of `ubatch` items
+ * and `bytes` bytes from the host-fed ring into the first stage's ring (one kernel; plus two stamp kernels with stamps
+ * on), filed as (ubatch, dim1, bit-width 0). pe_pipe_submit, pe_pipe_close_input, pe_pipe_next_result and pe_pipe_sync
+ * then work as for a data rank that owns the first stage. */
+int pe_pipe_capture_relay(pe_pipe* pipe, int ubatch, long long dim1, size_t bytes, int* kernels);
 int pe_pipe_capture_end(pe_pipe* pipe, const void* a0, const void* b0, size_t n0, const void* a1, const void* b1,
                         size_t n1, int items, int bit, int clamp, int overlap, int* kernels);
 int pe_pipe_capture_abort(pe_pipe* pipe);

@@ -106,6 +106,7 @@ SYMBOLS = {
     'pe_pipe_capture_begin': (c_int, [c_void_p, c_int, c_longlong, c_int, c_void_p, c_void_p, c_size_t, c_size_t, c_size_t]),
     'pe_pipe_capture_end': (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_size_t, c_int, c_int,
                                     c_int, c_int, POINTER(c_int)]),
+    'pe_pipe_capture_relay': (c_int, [c_void_p, c_int, c_longlong, c_size_t, POINTER(c_int)]),
     'pe_pipe_capture_abort': (c_int, [c_void_p]),
     'pe_pipe_invalidate': (c_int, [c_void_p]),
     'pe_pipe_set_out_dim': (c_int, [c_void_p, c_longlong]),

@@ -775,7 +775,8 @@ class DistP2pPipelineStage:
     # ------------------------------------------------------------------ native pipeline selection
     def _native_capable(self) -> bool:
         """Whether THIS rank's role can run on the native pipeline (csrc/pipe.cu): a native shard as the worker, hooks
-        that the link kernels account for, the reference's ring topology with the data rank on the first stage."""
+        that the link kernels account for, the reference's ring topology with the data rank on the first stage - or the
+        data rank outside the stage pipeline (no worker, both ranks set), which feeds the first stage through a relay."""
         rank_src, rank_dst, work_cb, results_cb = self._args
         if os.environ.get('PIPEEDGE_NATIVE', '1') == '0' or not torch.cuda.is_available():
             return False
@@ -785,14 +786,15 @@ class DistP2pPipelineStage:
             from ._native import shard_is_native   # pylint: disable=import-outside-toplevel
         except ImportError:
             return False
-        if work_cb is None or not shard_is_native(work_cb):
+        feeder = work_cb is None and results_cb is not None and rank_src is not None and rank_dst is not None
+        if not feeder and (work_cb is None or not shard_is_native(work_cb)):
             return False
         if any(thr._pre_hooks or thr._post_hooks   # pylint: disable=protected-access
                for thr in self._threads.values() if isinstance(thr, AbstractTensorExchangeThread)):
             return False   # user hooks run on the Python exchange threads (send-timing hooks do not: device timestamps)
         if (rank_src is None) != (rank_dst is None):
             return False
-        if results_cb is not None and not work_cb.shard_config.is_first:
+        if results_cb is not None and not feeder and not work_cb.shard_config.is_first:
             return False
         return True
 
@@ -838,6 +840,10 @@ class DistP2pPipelineStage:
             if work_cb is not None:
                 from ._native import NativeStage   # pylint: disable=import-outside-toplevel
                 self._native = NativeStage(rank_src, rank_dst, work_cb, results_cb)
+            elif results_cb is not None:   # the data rank outside the stage pipeline
+                from ._native import NativeFeeder   # pylint: disable=import-outside-toplevel
+                self._native = NativeFeeder(rank_src, rank_dst, results_cb)
+            if self._native is not None:
                 send = self._threads.get('send')
                 for hook, args in (send._timing_hooks if send is not None else ()):   # pylint: disable=protected-access
                     self._native.add_send_timing_hook(hook, args)   # registered before init(): stamps from the start
@@ -927,7 +933,8 @@ class DistP2pPipelineStage:
 
     @property
     def native(self):
-        """The `_native.NativeStage` driving this rank, or None (Python threads / idle rank)."""
+        """The `_native.NativeStage` driving this rank (a `_native.NativeFeeder` on a data rank outside the stage
+        pipeline), or None (Python threads / idle rank)."""
         return self._native
 
     def prepare(self, ubatch: int, dim1: int = 0) -> None:

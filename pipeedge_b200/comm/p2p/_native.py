@@ -6,7 +6,11 @@ per-micro-batch host work runs in C with the GIL released:
 
 * data rank: `enqueue_tensor` -> `pe_pipe_submit` (copy into the host-fed input ring on a side stream, graph launch,
   ticket to the next rank); a results thread blocks in `pe_pipe_next_result` and calls `results_cb` with each result;
-* other ranks: one thread sits in `pe_pipe_run` (ticket in -> graph launch -> ticket out) until the pipeline closes.
+* other ranks: one thread sits in `pe_pipe_run` (ticket in -> graph launch -> ticket out) until the pipeline closes;
+* a data rank outside the stage pipeline (`NativeFeeder`) owns no shard: its graph is one relay kernel that moves each
+  input micro-batch, bytes unchanged, from its host-fed ring into the first stage's ring (`pe_pipe_capture_relay`);
+  the first stage receives it as a raw payload from a peer link. The first stage tells the feeder its input geometry
+  over their hop's socket before the link opens (`send_input_geometry`).
 
 Activations cross hops as peer-memory stores synchronised by device-polled flags (`csrc/link.cu`); QuantPipe
 quantisation (`-q`, the shard's `quant_bit` buffer) is fused into the send kernel and undone by the receive kernel, so
@@ -27,6 +31,7 @@ import collections
 import ctypes
 import logging
 import os
+import struct
 import threading
 import time
 from typing import Callable, Iterable, List, NamedTuple, Optional, Set, Tuple
@@ -128,6 +133,46 @@ def payload_fits(room: int, items: int, elems: Iterable[int], bit: int, wire: in
     return True
 
 
+# Input geometry the first stage announces to a data rank outside the stage pipeline, on their hop's socket before the
+# link opens: magic | the largest input micro-batch in bytes | dtype name (NUL-padded) | tensor rank.
+_GEOMETRY = struct.Struct('<4sQ16sI')
+_GEOMETRY_MAGIC = b'PEIN'
+_INPUT_DTYPES = {'float32': torch.float32, 'int64': torch.int64}   # images, token ids
+
+
+def max_input_geometry(shard) -> Tuple[int, torch.dtype, int]:
+    """(bytes, dtype, tensor rank) of the largest input micro-batch a first-stage shard takes: `PIPEEDGE_MAX_UBATCH`
+    items of its longest sequence."""
+    shape, dtype = shard.native_input_spec(max_ubatch(), shard.native_max_tokens())[0]
+    nbytes = torch.empty((), dtype=dtype).element_size()
+    for d in shape:
+        nbytes *= int(d)
+    return nbytes, dtype, len(shape)
+
+
+def send_input_geometry(sock, nbytes: int, dtype: torch.dtype, ndim: int) -> None:
+    """First stage -> data rank outside the stage pipeline: what its input micro-batches look like."""
+    name = str(dtype).split('.')[-1]
+    if _INPUT_DTYPES.get(name) != dtype:
+        raise ValueError(f"native pipeline: input dtype {dtype} cannot be announced to the data rank")
+    sock.sendall(_GEOMETRY.pack(_GEOMETRY_MAGIC, nbytes, name.encode(), ndim))
+
+
+def recv_input_geometry(sock) -> Tuple[int, torch.dtype, int]:
+    """The data rank's side of `send_input_geometry`: (largest input in bytes, dtype, tensor rank)."""
+    buf = b''
+    while len(buf) < _GEOMETRY.size:
+        chunk = sock.recv(_GEOMETRY.size - len(buf))
+        if not chunk:
+            raise ConnectionError("native pipeline: the first stage closed its hop before announcing its input")
+        buf += chunk
+    magic, nbytes, name, ndim = _GEOMETRY.unpack(buf)
+    dtype = _INPUT_DTYPES.get(name.rstrip(b'\0').decode(errors='replace'))
+    if magic != _GEOMETRY_MAGIC or dtype is None or nbytes == 0 or ndim == 0:
+        raise ConnectionError("native pipeline: malformed input geometry from the first stage")
+    return nbytes, dtype, ndim
+
+
 class RecordShapeError(LookupError):
     """A timestamp record matches no payload shape the stage has captured (or more than one)."""
 
@@ -214,13 +259,16 @@ class RecordDrain:
 
 class NativeStage:
     """One rank's stage on the native pipeline. `rank_src` / `rank_dst` as `DistP2pPipelineStage`; the data rank is the
-    one with a `results_cb` (it must own the first shard)."""
+    one with a `results_cb` (here it owns the first shard; `NativeFeeder` is a data rank that owns none). A first stage
+    that is not the data rank receives its input relayed from a `NativeFeeder`."""
 
     def __init__(self, rank_src: Optional[int], rank_dst: Optional[int], shard, results_cb: Optional[Callable]):
         self._rank_src, self._rank_dst = rank_src, rank_dst
         self._shard = shard
         self._results_cb = results_cb
         self._is_data = results_cb is not None
+        # fed by a data rank outside the stage pipeline: a raw input payload arrives on the peer link
+        self._raw_in = shard is not None and shard.shard_config.is_first and not self._is_data and rank_src is not None
         self._device = torch.cuda.current_device()
         self._pipe = ctypes.c_void_p()
         self._links = []                      # every pe_link this rank opened (closed at shutdown)
@@ -240,7 +288,7 @@ class NativeStage:
         self._quant_cache = (None, 0, 0)      # (quant_bit tensor, its in-place version, its value)
         # Adaptive bit-widths: S = the initial bit-width | every set the shard's hooks declare; one graph per member
         bit0 = self._quant()[0]
-        declared = set() if shard.shard_config.is_last else declared_send_bits(shard)
+        declared = set() if shard is None or shard.shard_config.is_last else declared_send_bits(shard)
         self._send_bits = sorted(declared | {bit0})
         self.adaptive = len(self._send_bits) > 1
         self._pushed_bit = None               # the last pe_pipe_set_send_bit (by one thread: enqueue's or the drain's)
@@ -285,13 +333,12 @@ class NativeStage:
             else:
                 sock = accept_from(self._rank_src)
                 self._socks.append(sock)
+                if self._raw_in:   # the feeder owns no shard: it sizes the link from this
+                    send_input_geometry(sock, *max_input_geometry(shard))
                 peer_in = self._open_link(sock, False, 0)
         if self._is_data:
             # inputs arrive from the host; results come back on the hop from the last stage (or a loop-back link)
-            spec_shape, spec_dtype = shard.native_input_spec(ub, tokens)[0]
-            in_bytes = torch.empty((), dtype=spec_dtype).element_size()
-            for d in spec_shape:
-                in_bytes *= int(d)
+            in_bytes = max_input_geometry(shard)[0]
             handle = ctypes.c_void_p()
             check(LIB.pe_link_open_host(in_bytes, link_slots(), ctypes.byref(handle)))
             self._links.append(handle)
@@ -404,7 +451,7 @@ class NativeStage:
         last stage. The tensor is converted once per object / in-place version, never per micro-batch (a CUDA-resident
         buffer would cost a device synchronisation each time)."""
         shard = self._shard
-        if shard.shard_config.is_last or not hasattr(shard, 'quant_bit'):
+        if shard is None or shard.shard_config.is_last or not hasattr(shard, 'quant_bit'):
             return 0, _lib.PE_CLAMP_NONE
         qb = shard.quant_bit
         version = getattr(qb, '_version', 0)
@@ -494,7 +541,7 @@ class NativeStage:
             self._stream.synchronize()
             if check_slots and parity == 0:
                 self._check_slot_fits(parts, ubatch)
-            if self._is_data:
+            if self._is_data or self._raw_in:   # host-fed, or relayed unchanged by a data rank outside the pipeline
                 raw = ins[0].numel() * ins[0].element_size()
                 check(LIB.pe_pipe_capture_begin(self._pipe, ubatch, dim1, parity, ins[0].data_ptr(), None, 0, 0, raw))
             else:
@@ -550,9 +597,10 @@ class NativeStage:
             out = torch.frombuffer(buf, dtype=torch.float32, count=count).clone()
             shape = self._result_shape
             prod = 1
-            for d in shape:
+            for d in shape or ():
                 prod *= d
-            out = out.view(items.value, *shape) if prod == n.value else out.view(items.value, n.value)
+            out = out.view(items.value, *shape) if shape is not None and prod == n.value \
+                else out.view(items.value, n.value)
             self._results_cb(out)
 
     # ------------------------------------------------------------------ other ranks
@@ -624,3 +672,88 @@ class NativeStage:
                 pass
         self._socks.clear()
         self._inputs.clear()
+
+
+class NativeFeeder(NativeStage):
+    """A data rank outside the stage pipeline (`runtime.py -D <rank>` with the rank not in `-r`) on the native
+    pipeline: a stage without a shard. `enqueue` feeds its host-fed ring and launches its graph, ONE relay kernel that
+    moves the input micro-batch, bytes unchanged, into the first stage's ring; a results thread drains the last stage's
+    results as on a data rank that owns the first stage. `rank_dst`: the first stage; `rank_src`: the last stage."""
+
+    def __init__(self, rank_src: int, rank_dst: int, results_cb: Callable):
+        super().__init__(rank_src, rank_dst, None, results_cb)
+        self._geometry = None       # (largest input micro-batch in bytes, dtype, tensor rank) from the first stage
+        self._relay_bytes = {}      # (ubatch, dim1) -> input bytes its relay graph moves
+
+    def init(self, connect_to: Callable, accept_from: Callable) -> None:
+        """Open the hop to the first stage (reading its input geometry first) and the hop from the last one, in
+        ascending order of the sender's rank like every stage, then the host-fed ring; build the pipe."""
+        rank = dist.get_rank() if dist.is_initialized() else 0
+        peer_in = peer_out = None
+        for _, kind in sorted([(rank, 'send'), (self._rank_src, 'recv')]):
+            if kind == 'send':
+                sock = connect_to(self._rank_dst)
+                self._socks.append(sock)
+                self._geometry = recv_input_geometry(sock)
+                peer_out = self._open_link(sock, True, self._geometry[0])
+            else:
+                sock = accept_from(self._rank_src)
+                self._socks.append(sock)
+                peer_in = self._open_link(sock, False, 0)
+        handle = ctypes.c_void_p()
+        check(LIB.pe_link_open_host(self._geometry[0], link_slots(), ctypes.byref(handle)))
+        self._links.append(handle)
+        self._link_in, self._link_out, self._link_res = handle, peer_out, peer_in
+        check(LIB.pe_pipe_create(self._link_in, self._link_out, self._link_res, ctypes.byref(self._pipe)))
+        self._stream = torch.cuda.ExternalStream(LIB.pe_pipe_stream(self._pipe), device=self._device)
+        self._copy_stream = torch.cuda.ExternalStream(LIB.pe_pipe_copy_stream(self._pipe), device=self._device)
+        thr = threading.Thread(target=self._guard, args=(self._results_loop,), daemon=True, name='pe-results')
+        if self._send_hooks:
+            self._start_stamps()
+        self._threads.append(thr)
+        thr.start()
+
+    @property
+    def input_geometry(self) -> Optional[Tuple[int, torch.dtype, int]]:
+        """(largest input micro-batch in bytes, dtype, tensor rank) the first stage announced (after `init()`)."""
+        return self._geometry
+
+    def prepare(self, ubatch: int, dim1: int = 0) -> None:
+        """No-op: a relay graph is captured at a shape's first `enqueue` (its size comes from the tensor)."""
+
+    def enqueue(self, tensor: torch.Tensor) -> None:
+        """Insert one micro-batch (host or device tensor, converted to the first stage's input dtype); blocks while the
+        input ring is full."""
+        self.check()
+        max_bytes, dtype, ndim = self._geometry
+        if tensor.dim() != ndim:
+            raise ValueError(f"native pipeline: a {tensor.dim()}-D input where the first stage takes {ndim}-D ones")
+        ubatch = int(tensor.shape[0])
+        dim1 = int(tensor.shape[1]) if ndim == 2 else 0      # BERT: the sequence length is the payload's
+        if tensor.dtype != dtype or not tensor.is_contiguous():
+            tensor = tensor.to(dtype).contiguous()
+        nbytes = tensor.numel() * tensor.element_size()
+        if not LIB.pe_pipe_has_graph(self._pipe, ubatch, dim1):
+            self._capture_relay(ubatch, dim1, nbytes, max_bytes)
+        elif self._relay_bytes.get((ubatch, dim1)) != nbytes:
+            raise ValueError(f"native pipeline: an input of {nbytes} bytes where micro-batches of {ubatch} items "
+                             f"(dim {dim1}) had {self._relay_bytes.get((ubatch, dim1))}")
+        if tensor.is_cuda:
+            # the copy runs on the pipe's side stream: order it behind whatever produced the tensor
+            self._copy_stream.wait_event(torch.cuda.current_stream().record_event())
+        self._keep.append(tensor)
+        check(LIB.pe_pipe_submit(self._pipe, tensor.data_ptr(), nbytes, 0 if tensor.is_cuda else 1, ubatch, dim1))
+
+    def _capture_relay(self, ubatch: int, dim1: int, nbytes: int, max_bytes: int) -> None:
+        if ubatch > max_ubatch():
+            raise ValueError(f"micro-batch of {ubatch} items exceeds PIPEEDGE_MAX_UBATCH={max_ubatch()}")
+        if nbytes > max_bytes:
+            raise ValueError(f"native pipeline: an input of {nbytes} bytes exceeds the first stage's largest "
+                             f"({max_bytes} bytes)")
+        kernels = ctypes.c_int(0)
+        with self._capture_lock:
+            check(LIB.pe_pipe_capture_relay(self._pipe, ubatch, dim1, nbytes, ctypes.byref(kernels)))
+            self._relay_bytes[(ubatch, dim1)] = nbytes
+            self.graph_kernels[(ubatch, dim1)] = kernels.value
+            self.variant_kernels[(ubatch, dim1, 0)] = kernels.value
+            self.captures += 1

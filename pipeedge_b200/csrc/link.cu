@@ -13,7 +13,10 @@
 //                                        -> grid barrier -> clamp threshold, per-item scale / shift -> codes packed and
 //                                        stored into the peer slot, the fp32 slice kept in shared memory in between;
 //   get (consumer stage's first kernel)  waits for full[s], copies / dequantises the payload into the stage's fixed input
-//                                        buffer, raises free[s].
+//                                        buffer, raises free[s];
+//   relay (a data rank outside the       waits for its host-fed input slot and the first stage's free[s], copies the
+//   stage pipeline: its whole graph)     input bytes unchanged into that slot behind a raw header, raises full[s] and
+//                                        releases the host-fed slot.
 // Which slot a kernel works on comes from a device-resident sequence counter, so the kernels take no per-payload
 // arguments: a stage's whole micro-batch (get -> blocks -> put) is ONE CUDA graph replayed unchanged (pipe.cu).
 // The host side of a link is only a "ticket" per payload on the hop's Unix-domain socket, telling the consumer's host
@@ -95,9 +98,18 @@ struct GetArgs {
   size_t n0, n1;        // elements per item the stage expects (raw mode: n0 = bytes to copy)
   int items;
   int n_tensors;
-  int raw;              // host-fed link: no header, copy n0 bytes
+  int raw;              // copy n0 bytes: 1 = host-fed link (no header), 2 = relayed raw payload (header checked)
   unsigned long long timeout_ns;
 };
+
+__device__ __forceinline__ LinkHeader load_header(const uint8_t* base) {
+  LinkHeader h;
+  const uint4* src = reinterpret_cast<const uint4*>(base);
+  uint4* d = reinterpret_cast<uint4*>(&h);
+#pragma unroll
+  for (int i = 0; i < static_cast<int>(sizeof(LinkHeader) / 16); ++i) d[i] = __ldcg(src + i);
+  return h;
+}
 
 // Grid-stride copy with kU independent 16-byte loads in flight per thread (a lone load per trip left these kernels
 // latency-bound: ncu r02b measured 0.5 TB/s for a 4.8 MB payload).
@@ -216,6 +228,17 @@ __global__ void __launch_bounds__(kGetThreads) link_get_kernel(const GetArgs g) 
   const uint64_t slot = seq % static_cast<uint64_t>(g.rx.n_slots), k = seq / static_cast<uint64_t>(g.rx.n_slots);
   const uint8_t* base = g.rx.ring + slot * g.rx.slot_bytes;
   if (g.raw) {
+    if (g.raw == 2) {
+      const LinkHeader h = load_header(base);
+      if (h.magic != kLinkMagic || h.n_tensors != kLinkRawKind || h.t[0].dtype != kLinkDtypeBytes ||
+          h.items != static_cast<uint32_t>(g.items) || h.t[0].n != g.n0) {
+        if (threadIdx.x == 0)
+          printf("pipeedge_b200: raw payload mismatch: magic %x kind %u items %u bytes %llu (expected %d / %llu)\n",
+                 h.magic, h.n_tensors, h.items, static_cast<unsigned long long>(h.t[0].n), g.items,
+                 static_cast<unsigned long long>(g.n0));
+        fail(g.rx.status, kLinkErrHeader);
+      }
+    }
     const size_t tid = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
     const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
     const uint8_t* data = base + kLinkHeaderBytes;
@@ -226,14 +249,7 @@ __global__ void __launch_bounds__(kGetThreads) link_get_kernel(const GetArgs g) 
     for (size_t i = (n16 << 4) + tid; i < g.n0; i += stride)
       reinterpret_cast<uint8_t*>(g.dst0)[i] = __ldcg(data + i);
   } else {
-    const LinkHeader* hp = reinterpret_cast<const LinkHeader*>(base);
-    LinkHeader h;
-    {
-      const uint4* src = reinterpret_cast<const uint4*>(hp);
-      uint4* d = reinterpret_cast<uint4*>(&h);
-#pragma unroll
-      for (int i = 0; i < static_cast<int>(sizeof(LinkHeader) / 16); ++i) d[i] = __ldcg(src + i);
-    }
+    const LinkHeader h = load_header(base);
     const bool ok = h.magic == kLinkMagic && h.n_tensors == static_cast<uint32_t>(g.n_tensors) &&
                     h.items == static_cast<uint32_t>(g.items) && h.t[0].n == g.n0 &&
                     (g.n_tensors < 2 || h.t[1].n == g.n1);
@@ -545,6 +561,75 @@ __global__ void __launch_bounds__(kPutThreads, 1) link_put_quant_kernel(const Pu
   put_end(p, seq);
 }
 
+// ------------------------------------------------------------------------------------------------ relay
+// The data rank outside the stage pipeline owns no shard: its graph is this one kernel, which moves the next input
+// micro-batch from the host-fed ring (filled by link_feed on the copy stream) into the first stage's ring, with a raw
+// header the first stage's receive checks. Both rings' sequence counters advance together (one relay per payload).
+struct RelayArgs {
+  LinkRx rx;              // host-fed ring of this device
+  LinkTx tx;              // the first stage's ring (peer mapping)
+  size_t bytes;
+  int items;
+  unsigned long long timeout_ns;
+};
+
+__global__ void __launch_bounds__(kPutThreads) link_relay_kernel(const RelayArgs r) {
+  __shared__ uint64_t s_in, s_out;
+  if (threadIdx.x == 0) {
+    const uint64_t in_seq = *reinterpret_cast<volatile uint64_t*>(r.rx.seq);
+    const uint64_t out_seq = *reinterpret_cast<volatile uint64_t*>(r.tx.seq);
+    const uint64_t n_in = static_cast<uint64_t>(r.rx.n_slots), n_out = static_cast<uint64_t>(r.tx.n_slots);
+    spin_until_ge<32, 512>(r.rx.full + in_seq % n_in, in_seq / n_in + 1, r.timeout_ns, r.rx.status, kLinkErrWaitFull);
+    spin_until_ge<32, 512>(r.tx.free_ + out_seq % n_out, out_seq / n_out, r.timeout_ns, r.tx.status, kLinkErrWaitFree);
+    s_in = in_seq;
+    s_out = out_seq;
+  }
+  __syncthreads();
+  const uint64_t in_seq = s_in, out_seq = s_out;
+  const uint64_t in_slot = in_seq % static_cast<uint64_t>(r.rx.n_slots);
+  const uint64_t out_slot = out_seq % static_cast<uint64_t>(r.tx.n_slots);
+  const uint8_t* src = r.rx.ring + in_slot * r.rx.slot_bytes + kLinkHeaderBytes;
+  uint8_t* base = r.tx.ring + out_slot * r.tx.slot_bytes;
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    LinkHeader* h = reinterpret_cast<LinkHeader*>(base);
+    h->magic = kLinkMagic;
+    h->n_tensors = kLinkRawKind;
+    h->items = static_cast<uint32_t>(r.items);
+    h->pad = 0;
+    LinkTensorHdr th;
+    th.bit = 0;
+    th.dtype = kLinkDtypeBytes;
+    th.n = r.bytes;
+    th.data_off = kLinkHeaderBytes;
+    th.alpha = INFINITY;
+    th.pad = 0;
+    h->t[0] = th;
+  }
+  uint8_t* dst = base + kLinkHeaderBytes;
+  const size_t tid = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
+  const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
+  const size_t n16 = r.bytes >> 4;
+  const uint4* s4 = reinterpret_cast<const uint4*>(src);
+  uint4* d4 = reinterpret_cast<uint4*>(dst);
+  stream4(n16, tid, stride, [&](size_t i) { return __ldcg(s4 + i); }, [&](size_t i, uint4 v) { d4[i] = v; });
+  for (size_t i = (n16 << 4) + tid; i < r.bytes; i += stride) dst[i] = __ldcg(src + i);
+  // as put_end: one GPU-scope fence per CTA after its barrier; the last CTA to arrive publishes the peer slot and then
+  // hands the host-fed slot back (its free flag is link_feed's back-pressure)
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    const unsigned prev = atomicAdd(r.tx.done_ctr, 1u);
+    if (prev == gridDim.x - 1) {
+      *r.tx.done_ctr = 0;
+      *reinterpret_cast<volatile uint64_t*>(r.tx.seq) = out_seq + 1;
+      *reinterpret_cast<volatile uint64_t*>(r.rx.seq) = in_seq + 1;
+      __threadfence_system();
+      st_release_sys(r.tx.full + out_slot, out_seq / static_cast<uint64_t>(r.tx.n_slots) + 1);
+      st_release_sys(r.rx.free_ + in_slot, in_seq / static_cast<uint64_t>(r.rx.n_slots) + 1);
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ host helpers
 static unsigned long long default_timeout_ns() {
   const char* e = getenv("PIPEEDGE_LINK_TIMEOUT_S");
@@ -600,6 +685,7 @@ static void preload_kernels() {
   cudaFuncGetAttributes(&attr, link_wait_kernel);
   cudaFuncGetAttributes(&attr, link_put_copy_kernel);
   cudaFuncGetAttributes(&attr, link_put_staged_kernel);
+  cudaFuncGetAttributes(&attr, link_relay_kernel);
   cudaFuncGetAttributes(&attr, link_put_quant_kernel<2>);
   cudaFuncGetAttributes(&attr, link_put_quant_kernel<4>);
   cudaFuncGetAttributes(&attr, link_put_quant_kernel<8>);
@@ -853,19 +939,45 @@ int link_get(pe_link* l, void* dst0, void* dst1, int items, size_t n0, size_t n1
   return launch_get(l, g, static_cast<size_t>(items) * (n0 + g.n1) / 16, true, prewait, stream);
 }
 
-int link_get_raw(pe_link* l, void* dst, size_t bytes, cudaStream_t stream, bool prewait) {
+int link_get_raw(pe_link* l, void* dst, size_t bytes, int items, cudaStream_t stream, bool prewait) {
   PE_REQUIRE(l != nullptr && l->is_rx && dst != nullptr && bytes > 0, "pe_link_get_raw: bad arguments");
   PE_REQUIRE(kLinkHeaderBytes + bytes <= l->slot_bytes, "pe_link_get_raw: %zu bytes exceed the link's slots", bytes);
   PE_REQUIRE((reinterpret_cast<uintptr_t>(dst) & 15) == 0, "pe_link_get_raw: destination must be 16-byte aligned");
+  PE_REQUIRE(items >= 0 && items <= kLinkMaxItems && (items == 0 || l->kind != 2),
+             "pe_link_get_raw: a relayed raw payload (%d items) comes from a peer, not a host-fed link", items);
   GetArgs g = {};
   g.rx = l->rx;
   g.dst0 = dst;
   g.n0 = bytes;
-  g.items = 1;
+  g.items = items > 0 ? items : 1;
   g.n_tensors = 1;
-  g.raw = 1;
+  g.raw = items > 0 ? 2 : 1;
   g.timeout_ns = l->timeout_ns;
   return launch_get(l, g, bytes / 64, false, prewait, stream);
+}
+
+int link_relay(pe_link* in, pe_link* out, int items, size_t bytes, cudaStream_t stream) {
+  PE_REQUIRE(in != nullptr && in->kind == 2 && out != nullptr && out->is_tx,
+             "link_relay: needs a host-fed input and the producer end of a link");
+  PE_REQUIRE(items > 0 && items <= kLinkMaxItems && bytes > 0, "link_relay: %d items / %zu bytes outside [1,%d] / > 0",
+             items, bytes, kLinkMaxItems);
+  PE_REQUIRE(kLinkHeaderBytes + bytes <= in->slot_bytes && kLinkHeaderBytes + bytes <= out->slot_bytes,
+             "link_relay: %zu bytes exceed the input ring's %zu-byte or the link's %zu-byte slots", bytes,
+             in->slot_bytes - kLinkHeaderBytes, out->slot_bytes - kLinkHeaderBytes);
+  RelayArgs r = {};
+  r.rx = in->rx;
+  r.tx = out->tx;
+  r.bytes = bytes;
+  r.items = items;
+  r.timeout_ns = out->timeout_ns;
+  // the copy path's rule (plan_put): one 16-byte vector per thread, at most half the SMs
+  const size_t want = (bytes / 16 + kPutThreads - 1) / kPutThreads;
+  const size_t cap = static_cast<size_t>((sm_count() + 1) / 2);
+  const int grid = static_cast<int>(want < 1 ? 1 : (want > cap ? cap : want));
+  link_relay_kernel<<<grid, kPutThreads, 0, stream>>>(r);
+  PE_CUDA(cudaGetLastError());
+  count_launches(1);
+  return PE_OK;
 }
 
 // Host-fed link: copy the next payload into the ring (waiting for its slot to be released) and raise its flag, both on
@@ -1155,7 +1267,7 @@ int pe_link_get(pe_link* link, void* dst0, void* dst1, int items, size_t n0, siz
 }
 
 int pe_link_get_raw(pe_link* link, void* dst, size_t bytes, void* stream) {
-  return pe::link_get_raw(link, dst, bytes, static_cast<cudaStream_t>(stream), true);
+  return pe::link_get_raw(link, dst, bytes, 0, static_cast<cudaStream_t>(stream), true);
 }
 
 int pe_link_feed(pe_link* link, const void* src, size_t bytes, int src_is_host, void* copy_stream) {

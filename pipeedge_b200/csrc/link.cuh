@@ -38,6 +38,10 @@ struct LinkHeader {        // first bytes of every slot that carries activations
   uint32_t pad;
   LinkTensorHdr t[2];
 };
+// A raw payload (the data rank's input micro-batch relayed to the first stage, link_relay): n_tensors = kLinkRawKind,
+// t[0].n = bytes, t[0].dtype = kLinkDtypeBytes, bit 0, the bytes at kLinkHeaderBytes, unconverted.
+constexpr uint32_t kLinkRawKind = 0;
+constexpr uint32_t kLinkDtypeBytes = 2;
 
 // Receiver-side view of a link (what a get kernel dereferences). All flags are monotonic counters: slot s is used for
 // payloads s, s + R, s + 2R, ...; its k-th use is complete when full[s] == k + 1 and may be overwritten when
@@ -119,7 +123,11 @@ int link_put(pe_link* link, const PutTensor* t, int n_tensors, int items, int bi
 // prewait: park in the one-warp wait kernel first (consumers that may wait long while other streams compute)
 int link_get(pe_link* link, void* dst0, void* dst1, int items, size_t n0, size_t n1, int n_tensors, cudaStream_t stream,
              bool prewait);
-int link_get_raw(pe_link* link, void* dst, size_t bytes, cudaStream_t stream, bool prewait);
+// items == 0: headerless (a host-fed link); items > 0: a raw payload relayed from a peer (link_relay) whose header must
+// name `bytes` and `items`
+int link_get_raw(pe_link* link, void* dst, size_t bytes, int items, cudaStream_t stream, bool prewait);
+// Data rank outside the stage pipeline: the next host-fed payload of `in` (`bytes`, `items`) -> the peer ring of `out`
+int link_relay(pe_link* in, pe_link* out, int items, size_t bytes, cudaStream_t stream);
 int link_feed(pe_link* link, const void* src, size_t bytes, int src_is_host, cudaStream_t copy_stream);
 int link_ticket_send(pe_link* link, long long a, long long b);
 int link_ticket_recv(pe_link* link, long long* out2);   // 0 ok, 1 = peer closed

@@ -8,7 +8,9 @@
 //     read a 16-byte ticket from the upstream hop's socket (blocks) -> cudaGraphLaunch -> write the ticket downstream
 // i.e. two system calls and one launch per micro-batch; ordering against the neighbours' GPUs is entirely on the
 // devices (flags in peer memory). The data rank feeds its first stage through a host-fed link (pe_pipe_submit: H2D /
-// D2D copy on a side stream + graph launch) and drains results through pe_pipe_next_result.
+// D2D copy on a side stream + graph launch) and drains results through pe_pipe_next_result. A data rank outside the
+// stage pipeline does the same with a graph of one relay kernel (pe_pipe_capture_relay) that forwards the fed input to
+// the first stage, whose graph then starts with a raw receive from its peer link.
 //
 // Replaces TensorWorkThread.run + the queue hand-offs of DistP2pPipelineStage (p2p/__init__.py:261-295,373-394,442-450):
 // FIFO per hop (tickets and flags are strictly ordered), back-pressure through the rings (a producer blocks - on the
@@ -243,6 +245,35 @@ static void destroy_graph(pe_pipe::Graph& g) {
   g.n_par = 0;
 }
 
+// File a captured graph (one parity of it) under (ubatch, dim1, bit).
+static void file_graph(pe_pipe* p, int ubatch, long long dim1, int bit, int par, cudaGraphExec_t exec_main,
+                       cudaGraphExec_t exec_put, int want_par, int kernels, bool stamps) {
+  std::lock_guard<std::mutex> lock(p->graphs_mu);
+  pe_pipe::Graph& g = p->graphs[std::make_tuple(ubatch, dim1, bit)];
+  if (par == 0) {   // a fresh capture of this key starts with parity 0
+    destroy_graph(g);
+    p->latest_bit[std::make_pair(ubatch, dim1)] = bit;
+    if (p->send_bit.load() < 0) {
+      // no bit-width selected: the capture replaces the shape's graph, whatever bit-width that one sent with
+      for (auto it = p->graphs.lower_bound(std::make_tuple(ubatch, dim1, INT_MIN));
+           it != p->graphs.end() && std::get<0>(it->first) == ubatch && std::get<1>(it->first) == dim1;) {
+        if (std::get<2>(it->first) == bit) {
+          ++it;
+          continue;
+        }
+        destroy_graph(it->second);
+        it = p->graphs.erase(it);
+      }
+    }
+  }
+  g.want_par = want_par;
+  g.exec[par] = exec_main;
+  g.exec_put[par] = exec_put;
+  g.n_par = par + 1;
+  g.kernels = kernels;
+  g.stamps = stamps;
+}
+
 static int launch_graph(pe_pipe* p, int ubatch, long long dim1, int bit) {
   pe_pipe::Graph g;
   PE_REQUIRE(find_graph(p, ubatch, dim1, bit, &g, false),
@@ -385,7 +416,8 @@ int pe_pipe_set_send_bit(pe_pipe* p, int bit) {
 
 // Start capturing the graph for micro-batches of `ubatch` items (`dim1`: sequence length, part of the key). The get
 // kernel is enqueued first: from a host-fed link `raw_bytes` bytes land in dst0; from a hop the payload's one or two
-// tensors ([ubatch, n0] / [ubatch, n1] f32 after decoding) land in dst0 / dst1.
+// tensors ([ubatch, n0] / [ubatch, n1] f32 after decoding) land in dst0 / dst1, or, with raw_bytes > 0 (the first stage
+// fed by a data rank outside the stage pipeline, pe_pipe_capture_relay), the relayed input's `raw_bytes` bytes.
 int pe_pipe_capture_begin(pe_pipe* p, int ubatch, long long dim1, int parity, void* dst0, void* dst1, size_t n0, size_t n1,
                           size_t raw_bytes) {
   using namespace pe;
@@ -410,12 +442,13 @@ int pe_pipe_capture_begin(pe_pipe* p, int ubatch, long long dim1, int parity, vo
   st.what = kStampStart;
   int rc = p->cap_stamps ? launch_stamp(p, st, p->compute) : PE_OK;
   if (rc == PE_OK) {
-    if (p->in->kind == 2) rc = link_get_raw(p->in, dst0, raw_bytes, p->compute, false);
+    if (p->in->kind == 2) rc = link_get_raw(p->in, dst0, raw_bytes, 0, p->compute, false);
+    else if (raw_bytes > 0) rc = link_get_raw(p->in, dst0, raw_bytes, ubatch, p->compute, false);   // from a relay
     else rc = link_get(p->in, dst0, dst1, ubatch, n0, n1, dst1 != nullptr ? 2 : 1, p->compute, false);
   }
   if (rc == PE_OK && p->cap_stamps) {
     st.what = kStampGot;
-    if (p->in->kind != 2) {
+    if (p->in->kind != 2 && raw_bytes == 0) {   // a raw input was not quantised: bit_in stays -1
       st.in_ring = p->in->rx.ring;
       st.in_slot_bytes = p->in->rx.slot_bytes;
       st.in_slots = p->in->rx.n_slots;
@@ -518,35 +551,54 @@ int pe_pipe_capture_end(pe_pipe* p, const void* a0, const void* b0, size_t n0, c
     }
   }
   const int captured = static_cast<int>(launch_count_now() - p->cap_launch0);
-  int total = captured;
-  {
-    std::lock_guard<std::mutex> lock(p->graphs_mu);
-    pe_pipe::Graph& g = p->graphs[std::make_tuple(p->cap_ubatch, p->cap_dim1, bit)];
-    if (par == 0) {   // a fresh capture of this key starts with parity 0
-      destroy_graph(g);
-      p->latest_bit[std::make_pair(p->cap_ubatch, p->cap_dim1)] = bit;
-      if (p->send_bit.load() < 0) {
-        // no bit-width selected: the capture replaces the shape's graph, whatever bit-width that one sent with
-        for (auto it = p->graphs.lower_bound(std::make_tuple(p->cap_ubatch, p->cap_dim1, INT_MIN));
-             it != p->graphs.end() && std::get<0>(it->first) == p->cap_ubatch && std::get<1>(it->first) == p->cap_dim1;) {
-          if (std::get<2>(it->first) == bit) {
-            ++it;
-            continue;
-          }
-          destroy_graph(it->second);
-          it = p->graphs.erase(it);
-        }
-      }
-    }
-    g.want_par = overlap != 0 ? 2 : 1;
-    g.exec[par] = exec_main;
-    g.exec_put[par] = exec_put;
-    g.n_par = par + 1;
-    g.kernels = captured;
-    g.stamps = stamps;
-    total = g.kernels;
+  file_graph(p, p->cap_ubatch, p->cap_dim1, bit, par, exec_main, exec_put, overlap != 0 ? 2 : 1, captured, stamps);
+  if (kernels != nullptr) *kernels = captured;
+  return PE_OK;
+}
+
+// Data rank outside the stage pipeline (in: host-fed link, out: the producer end of the hop to the first stage, res: the
+// consumer end of the hop from the last stage): capture the relay graph of micro-batches of `ubatch` items whose input
+// is `bytes` bytes, filed as (ubatch, dim1, bit-width 0). pe_pipe_submit / close_input / next_result / sync then serve
+// it as they serve a data rank that owns the first stage. With stamps on, the graph's record has t_start, t_send_start,
+// t_send_end, bytes_out = `bytes`, bit_out = 0 and bit_in = -1. *kernels = kernels per micro-batch.
+int pe_pipe_capture_relay(pe_pipe* p, int ubatch, long long dim1, size_t bytes, int* kernels) {
+  using namespace pe;
+  PE_REQUIRE(p != nullptr && !p->capturing, "pe_pipe_capture_relay: bad state");
+  PE_REQUIRE(p->in->kind == 2, "pe_pipe_capture_relay: this pipe's input is not host-fed");
+  PE_REQUIRE(ubatch > 0 && ubatch <= kLinkMaxItems && bytes > 0, "pe_pipe_capture_relay: %d items / %zu bytes", ubatch,
+             bytes);
+  PE_REQUIRE(kLinkHeaderBytes + bytes <= p->in->slot_bytes && kLinkHeaderBytes + bytes <= p->out->slot_bytes,
+             "pe_pipe_capture_relay: %zu bytes exceed the input ring's %zu-byte or the link's %zu-byte slots", bytes,
+             p->in->slot_bytes - kLinkHeaderBytes, p->out->slot_bytes - kLinkHeaderBytes);
+  PE_CUDA(cudaStreamSynchronize(p->compute));
+  const bool stamps = p->stamps_on.load();
+  PE_CUDA(cudaStreamBeginCapture(p->compute, cudaStreamCaptureModeRelaxed));
+  p->capturing = true;
+  StampArgs st = {};
+  st.what = kStampStart | kStampGot | kStampStage | kStampSendStart;   // no receive, no stage: one stamp
+  int rc = stamps ? launch_stamp(p, st, p->compute) : PE_OK;
+  if (rc == PE_OK) rc = link_relay(p->in, p->out, ubatch, bytes, p->compute);
+  if (rc == PE_OK && stamps) {
+    st = {};
+    st.what = kStampSendEnd;
+    st.bump = 3;
+    st.items = ubatch;
+    st.bit_out = 0;
+    st.bytes_out = bytes;
+    rc = launch_stamp(p, st, p->compute);
   }
-  if (kernels != nullptr) *kernels = total;
+  if (rc != PE_OK) {
+    pe_pipe_capture_abort(p);
+    return rc;
+  }
+  p->capturing = false;
+  cudaGraphExec_t exec = nullptr;
+  rc = end_capture(p->compute, &exec, "cudaStreamEndCapture (relay)");
+  if (rc != PE_OK) return rc;
+  // counted here, not from the process-wide launch counter: the results thread may launch receives meanwhile
+  const int captured = stamps ? 3 : 1;
+  file_graph(p, ubatch, dim1, 0, 0, exec, nullptr, 1, captured, stamps);
+  if (kernels != nullptr) *kernels = captured;
   return PE_OK;
 }
 

@@ -577,6 +577,8 @@ def run_pipeline_p2p(world_size: int, rank: int, model_name: str, model_file: Op
                                                        handle_results) as stage_ctx:
             if model is not None:
                 logger.info("Pipeline stage: %s", 'native' if stage_ctx.native is not None else 'Python threads')
+            elif rank == data_rank:   # outside the stage pipeline: it feeds the first stage and collects results
+                logger.info("Data rank: %s", 'native' if stage_ctx.native is not None else 'Python threads')
             if os.getenv(ENV_ADAPTIVE_QUANT) or monitoring_enabled():
                 stage_ctx.register_send_timing_hook(hop_timing_hook_monitor, (MONITORING_KEY_SEND,))
             if rank == data_rank:
