@@ -232,6 +232,13 @@ __device__ __forceinline__ float2 ld_dsmem_f2(uint32_t cluster_addr) {
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_bar_addr) {
   asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar_addr) : "memory");
 }
+// arrive on an mbarrier of another CTA of the cluster with the default CTA-scope release: for a consumer handing a ring
+// stage back to the CTA that refills it, where the only order needed (its reads of the stage are done) comes from the
+// wgmma.wait_group before it. The cluster-scope release above makes every arrival wait for this CTA's outstanding
+// memory operations to become visible cluster-wide, which stalls the releasing warp once per stage.
+__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_bar_addr) {
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar_addr) : "memory");
+}
 // wait on this CTA's mbarrier with cluster-scope acquire (pairs with mbar_arrive_cluster); bounded like mbar_wait_addr
 // and without a printf, which would be a function call that serialises the caller's wgmma pipeline
 __device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {

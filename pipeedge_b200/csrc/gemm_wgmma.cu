@@ -14,7 +14,8 @@
 // TMA-MULTICAST it to the others, likewise the CN CTAs sharing an A tile, cutting L2 reads by up to CM (W) and CN (A).
 // Every CTA's `full` barrier sees the bytes of its whole stage whoever issued them; each consumer warpgroup releases a
 // stage to all of its writers (remote mbarrier arrivals). The fused projection + residual + LayerNorm uses clusters
-// to give one row's column slices to the CN CTAs of a cluster; pe_linear plans single CTAs (see plan_gemm).
+// to give one row's column slices to the CN CTAs of a cluster; pe_linear plans 1 x 2 clusters for some long-K GEMMs
+// (plan_gemm).
 //
 // Replaces every nn.Linear on the reference path (see include/pipeedge_b200.h: pe_linear).
 #include <math.h>
@@ -370,7 +371,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
         wgmma_wait<1>();   // the previous stage's wgmmas have retired: it may be refilled
         if (prev_stage >= 0 && releaser) {
           const uint32_t e = empty_remote0 + static_cast<uint32_t>(prev_stage) * 8u;
-          if (csize > 1) mbar_arrive_cluster(e);
+          if (csize > 1) mbar_arrive_remote(e);
           else mbar_arrive_addr(e);
         }
         prev_stage = stage;
@@ -379,7 +380,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
       wgmma_wait<0>();
       if (releaser) {
         const uint32_t e = empty_remote0 + static_cast<uint32_t>(prev_stage) * 8u;
-        if (csize > 1) mbar_arrive_cluster(e);
+        if (csize > 1) mbar_arrive_remote(e);
         else mbar_arrive_addr(e);
       }
       if (trace != nullptr && sup == cluster_id && threadIdx.x == 0) trace[3] = clock64();
@@ -554,8 +555,13 @@ static int max_clusters(int csize) {
 //   epilogue of a 128 x BN tile ~800 + c*BN, c growing with the per-element work (GELU and tanh are MUFU / issue bound);
 //   tiles are dealt round-robin to <= 132 CTAs; the accumulators live in registers, so a CTA's epilogue is not hidden
 //     under its next tile's MMAs (the producers only prefetch that tile's first stages).
-// Clusters cut L2 reads but are not L2-bound at these shapes, so pe_linear plans single CTAs; PE_GEMM_FORCE="CM,CN,BN"
-// selects any plan (tuning and tests).
+// L2 term, for single-wave plans with a long K loop (>= 32 blocks) only: there every CTA streams its A block and W
+// panel once, and the launch takes about its operand bytes over the L2 -> SM rate (measured on H100,
+// scripts/gemm_cluster_sweep.py, DESIGN.md 4a: ~6.5-7.6 TB/s for single CTAs, ~5.6 TB/s for pairs that multicast A).
+// A 1 x 2 cluster halves the A reads; it pays when that cuts a tile's bytes (128 + BN rows) by more than the rate
+// lost, i.e. to < 0.75 (ViT-B FC2, BN 96: 0.71, 22.0 -> 18.2 us; BERT-base FC2, BN 192: 0.80, 33.1 -> 35.4 us).
+// Pairs only: larger clusters measured no better at ViT-B FC2, and some of their single-wave grids ran at twice the
+// time, as if they did not all fit on the GPCs at once. PE_GEMM_FORCE="CM,CN,BN" selects any plan (tuning and tests).
 GemmPlan plan_gemm(int m, int n, int k, int epilogue) {
   int forced[3] = {0, 0, 0};
   const char* env = getenv("PE_GEMM_FORCE");
@@ -575,6 +581,9 @@ GemmPlan plan_gemm(int m, int n, int k, int epilogue) {
       best = {1, 1, bn};
     }
   }
+  const int m_blocks = (m + kBlockM - 1) / kBlockM, n_blocks = (n + best.bn - 1) / best.bn;
+  const bool pairs_one_wave = static_cast<long>(m_blocks) * ((n_blocks + 1) / 2) <= max_clusters(2);
+  if (kb >= 32 && pairs_one_wave && (64.0 + best.bn) < 0.75 * (128.0 + best.bn)) best = {1, 2, best.bn};
   return best;
 }
 
