@@ -494,6 +494,29 @@ def layernorm_ref(x64, gamma, beta, eps, in_err=None, depth=LN_SUM_DEPTH):
     return y, bound
 
 
+def linear_ln_ref(a16, w16, bias, resid, gamma, beta, eps, c=C_GEMM):
+    """The fused projection + residual + LayerNorm epilogue (PE_EPI_RESID_LN): v = a w^T + bias + resid in fp64 with the
+    bound of the kernel's fp32 v (the GEMM's, the residual counted in the magnitude), and LayerNorm(v) with a bound that
+    takes that error as the LayerNorm's input error, plus the rounding of v itself. Returns (v, v_bound, ln, ln_bound)."""
+    x, mag = gemm_ref(a16, w16, bias, resid)
+    v = x + resid.double()
+    v_bound = c * U32 * mag
+    ln, ln_bound = layernorm_ref(v, gamma, beta, eps, in_err=v_bound + U32 * v.abs())
+    return v, v_bound, ln, ln_bound
+
+
+def check_linear_ln(got32, got16, a16, w16, bias, resid, gamma, beta, eps, f32_is_ln, c=C_GEMM, where=''):
+    """-> (report of the fp32 output, report of the fp16 output). The fp32 output is LayerNorm(v) when `f32_is_ln`, else
+    v held to the GEMM bound; the fp16 output must be a faithful rounding of LayerNorm(v). `resid` is the residual as it
+    was BEFORE the call (the kernel may write its fp32 output over it)."""
+    v, v_bound, ln, ln_bound = linear_ln_ref(a16, w16, bias, resid, gamma, beta, eps, c)
+    if f32_is_ln:
+        rep32 = check_f32(got32, ln, ln_bound, where + ' f32 = LayerNorm(v)')
+    else:
+        rep32 = check_f32(got32, v, v_bound, where + ' f32 = v')
+    return rep32, check_f16(got16, ln, ln - ln_bound, ln + ln_bound, where + ' f16')
+
+
 LN_KINDS = ('normal', 'offset', 'offset_1e4')
 
 

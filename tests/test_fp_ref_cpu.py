@@ -222,6 +222,36 @@ def test_layernorm_checker(kind):
         assert not R.check_f32(b.expand_as(x), ref, bound).passed
 
 
+@pytest.mark.parametrize('offset', [0.0, 1e3])
+def test_linear_ln_checker(offset):
+    """The fused projection + residual + LayerNorm check: an fp32 kernel (accumulate, + bias, + resid, two-pass
+    LayerNorm) passes with either fp32 output. Rejected: a LayerNorm of v without the residual, and (on rows offset by
+    1e3, where it cancels) a one-pass variance."""
+    m, n, k = 70, 192, 256
+    gen = torch.Generator().manual_seed(11)
+    a = (torch.randn(m, k, generator=gen) * 0.7).half()
+    w = (torch.randn(n, k, generator=gen) * (1.0 / math.sqrt(k))).half()
+    bias = torch.randn(n, generator=gen) * 0.1
+    resid = offset + torch.randn(m, n, generator=gen)
+    g = 1 + 0.1 * torch.randn(n, generator=gen)
+    b = 0.1 * torch.randn(n, generator=gen)
+    eps = 1e-12
+    x = a.float() @ w.float().t() + bias
+    v = x + resid
+    ln = _ln_fp32(v, g, b, eps)
+
+    def passes(got32, got16, f32_is_ln):
+        r32, r16 = R.check_linear_ln(got32, got16, a, w, bias, resid, g, b, eps, f32_is_ln)
+        return r32.passed and r16.passed
+
+    assert passes(v, ln.half(), False) and passes(ln, ln.half(), True)
+    no_resid = _ln_fp32(x, g, b, eps)
+    assert not passes(v, no_resid.half(), False) and not passes(no_resid, ln.half(), True)
+    if offset:
+        one_pass = _ln_fp32(v, g, b, eps, single_pass=True)
+        assert not passes(v, one_pass.half(), False) and not passes(one_pass, ln.half(), True)
+
+
 # ------------------------------------------------------------------------------------ GEMM case list coverage
 def _plan(case):
     from pipeedge_b200 import _lib

@@ -438,6 +438,49 @@ def test_layernorm_rejects_too_wide_rows(ops):
         ops.layernorm(x, g, g, 1e-12)
 
 
+# ------------------------------------------------------------------------- projection + residual + LayerNorm (fused)
+LINEAR_LN_CASES = [
+    # m, n, k, rows, cluster: 1 to 3 row tiles of 128 with ragged last ones, several tiles per cluster (4096 rows)
+    (128, 768, 768, 'normal', 8),
+    (300, 768, 3072, 'offset', 8),
+    (256, 1024, 4096, 'normal', 8),
+    (384, 384, 1536, 'offset', 4),
+    (70, 192, 768, 'normal', 2),
+    (200, 96, 512, 'offset', 1),
+    (4096, 768, 768, 'offset', 8),
+]
+
+
+@pytest.mark.parametrize('f32_is_ln', [False, True], ids=['f32=v', 'f32=ln'])
+@pytest.mark.parametrize('m,n,k,rows,cluster', LINEAR_LN_CASES, ids=lambda v: str(v))
+def test_linear_residual_layernorm(ops, m, n, k, rows, cluster, f32_is_ln):
+    """The fused epilogue (clusters of 8, 4, 2 and 1 CTAs exchanging row statistics) against fp64, its fp32 output
+    written over the residual in place as the stage does: LayerNorm(v) within the LayerNorm bound fed by the GEMM's
+    error, the fp16 output a faithful rounding of it, and v itself (f32_is_ln off) within the GEMM bound. 'offset'
+    rows sit at 1e3 + N(0, 1) (a one-pass variance cancels there)."""
+    assert _lib().LIB.pe_linear_ln_cluster(n) == cluster
+    gen = torch.Generator().manual_seed(m + n + k)
+    a = (torch.randn(m, k, generator=gen) * 0.7).half()
+    w = (torch.randn(n, k, generator=gen) * (1.0 / k ** 0.5)).half()
+    bias = torch.randn(n, generator=gen) * 0.1
+    resid = (1e3 if rows == 'offset' else 0.2) + torch.randn(m, n, generator=gen) * 1.3
+    gamma = 1.0 + 0.1 * torch.randn(n, generator=gen)
+    beta = 0.1 * torch.randn(n, generator=gen)
+    eps = 1e-12
+    dev = [t.cuda() for t in (a, w, bias, resid, gamma, beta)]
+    r_dev = dev[3]
+    o32, o16 = ops.linear_residual_layernorm(dev[0], dev[1], dev[2], r_dev, dev[4], dev[5], eps, f32_is_ln=f32_is_ln,
+                                             out_f32=r_dev)
+    torch.cuda.synchronize()
+    assert o32.data_ptr() == r_dev.data_ptr()
+    where = f'linear+ln {m}x{n}x{k} {rows} cluster {cluster}'
+    rep32, rep16 = R.check_linear_ln(o32, o16, dev[0], dev[1], dev[2], resid.cuda(), dev[4], dev[5], eps, f32_is_ln,
+                                     where=where)
+    v, _, ln, _ = R.linear_ln_ref(dev[0], dev[1], dev[2], resid.cuda(), dev[4], dev[5], eps)
+    _assert(rep32, o32, ln if f32_is_ln else v, 'linear-ln-f32-' + ('ln' if f32_is_ln else 'v'))
+    _assert(rep16, o16, ln, 'linear-ln-f16')
+
+
 def test_layernorm_fused_mirror(ops):
     """The same cases with PE_FUSE_LN=1 (child process): the chunked stand-alone kernel for the widths the fused
     projection supports, the two-pass kernel for the others."""
