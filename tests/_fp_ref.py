@@ -6,7 +6,8 @@ fp16 / fp32 operands, element by element, against an error bound derived from th
 tolerance. The CPU tests (`test_fp_ref_cpu.py`) show that each checker rejects plausible wrong kernels.
 
 Bounds (u = 2^-24, the fp32 unit roundoff):
-  * fp32 GEMM outputs: |got - ref| <= C u (sum_k |a_ik w_jk| + |b_j| + |resid_ij|).
+  * fp32 GEMM outputs: |got - ref| <= C u (sum_k |a_ik w_jk| + |b_j| + |resid_ij|) + 2 u sum_s |S_ij(s)|, S(s) the exact
+    partial sum after k-step s of K_STEP products (`gemm_ref`).
   * tanh epilogue: the same, propagated through tanh, plus 2 ulp of fp32 (CUDA's documented tanhf accuracy).
   * fp16 outputs: `got` is one of the two fp16 neighbours of some exact value within the fp32 bound ("faithful").
 """
@@ -18,9 +19,17 @@ import os
 import torch
 
 U32 = 2.0 ** -24
-# One constant for every GEMM shape, plan and epilogue: the fp32 accumulation error of the wgmma main loop plus the
-# epilogue's few roundings, in units of u * sum |a w|. Calibrated on an H100 (see the commit that introduced it).
+# One constant for every GEMM shape, plan and epilogue: the error of summing one wgmma instruction's products into the
+# accumulator plus the epilogue's few roundings, in units of u * sum |a w|. Calibrated on an H100 (see the commit that
+# introduced it) at K <= 776.
 C_GEMM = 16.0
+# k per wgmma instruction. The tensor cores add each instruction's 16 products to the fp32 accumulator with one
+# rounding that is not to nearest (it truncates): its errors do not cancel, they pile up with the number of
+# instructions, each at most 2 u of the partial sum it produces. With operands whose dot products drift one way (FC2
+# reads GELU outputs, which are mostly positive) that term grows about linearly in K: measured on an H100 SXM (700 W),
+# ViT-L's FC2 (K = 4096) reached 1.05 x the C u sum|a w| bound on 2 of 3.2 million outputs; with this term no
+# product GEMM of K >= 3072 comes above 0.30 x the bound.
+K_STEP = 16
 
 # epilogue ids, in the order of PE_EPI_* in include/pipeedge_b200.h (asserted by the tests)
 EPI = {'F16': 0, 'GELU_F16': 1, 'RESID_F32': 2, 'F32': 3, 'TANH_F32': 4}
@@ -161,6 +170,16 @@ def _gelu_range(lo, hi):
     return gmin, torch.maximum(glo, ghi)
 
 
+def partial_sums_magnitude(ad, wd, step=K_STEP):
+    """sum over the k-steps s of |S(s)|, S(s) = the exact a w^T over k < step * (s + 1) (float64 operands)."""
+    s = torch.zeros(ad.shape[0], wd.shape[0], dtype=torch.float64, device=ad.device)
+    total = torch.zeros_like(s)
+    for k0 in range(0, ad.shape[1], step):
+        s += ad[:, k0:k0 + step] @ wd[:, k0:k0 + step].t()
+        total += s.abs()
+    return total
+
+
 def gemm_ref(a16, w16, bias, resid):
     """(pre-activation x = a w^T + bias in fp64, magnitude sum|a w| + |bias| + |resid|) on the operands' device."""
     ad, wd = a16.double(), w16.double()
@@ -174,10 +193,16 @@ def gemm_ref(a16, w16, bias, resid):
     return x, mag
 
 
+def gemm_bound(a16, w16, mag, c=C_GEMM):
+    """The fp32 error bound of a GEMM output: C u per unit of `mag` (from gemm_ref) plus the truncating accumulation
+    of one wgmma instruction after the other (2 u of every partial sum, see K_STEP)."""
+    return c * U32 * mag + 2 * U32 * partial_sums_magnitude(a16.double(), w16.double())
+
+
 def check_gemm(epi: str, got, a16, w16, bias=None, resid=None, c=C_GEMM, where='') -> Report:
     """Check one pe_linear output. `resid` is the residual as it was BEFORE the call (for in-place RESID_F32)."""
     x, mag = gemm_ref(a16, w16, bias, resid if epi == 'RESID_F32' else None)
-    bound = c * U32 * mag
+    bound = gemm_bound(a16, w16, mag, c)
     if epi == 'F32':
         return check_f32(got, x, bound, where)
     if epi == 'RESID_F32':
@@ -234,14 +259,21 @@ FORCED_PLANS = ('1,1,32', '1,1,160', '2,1,64', '1,2,128', '2,2,128', '1,4,64', '
 SCHED_SHAPE = (1100, 1080, 776)      # 9 M blocks (odd), ragged K; N blocks odd for BN 128, not a multiple of 4 / 8 for 64 / 32
 
 
-def plan_geometry(plan6, m, n):
-    """pe_debug_gemm_plan's {cm, cn, block_n, stages, tiles, ctas} -> what decides the kernel's path."""
+def plan_geometry(plan6, m, n, k):
+    """pe_debug_gemm_plan's {cm, cn, block_n, stages, tiles, ctas} -> what decides the kernel's path: the cluster and
+    tile shape, the tiles of the busiest CTA (`rounds`; more than one puts the epilogue staging behind the ring instead
+    of aliasing it), partly empty clusters, the scalar epilogue, the ring depth, a K loop shorter than the ring
+    (`kb_lt_stages`) and whether every tile starts on ring slot 0 with the same barrier phase (`ring_repeats`:
+    k-blocks a multiple of the depth; otherwise a CTA's later tiles start mid-ring, or on the other phase)."""
     cm, cn, bn, stages, tiles, ctas = plan6
     mb, nb = -(-m // 128), -(-n // bn)
+    kb = -(-k // 64)
     supers = -(-mb // cm) * -(-nb // cn)
     clusters = ctas // (cm * cn)
-    return {'cm': cm, 'cn': cn, 'bn': bn, 'rounds': -(-supers // clusters), 'partial_m': mb % cm != 0,
-            'partial_n': nb % cn != 0, 'scalar': n % 8 != 0, 'tiles': tiles}
+    rounds = -(-supers // clusters)
+    return {'cm': cm, 'cn': cn, 'bn': bn, 'rounds': rounds, 'partial_m': mb % cm != 0,
+            'partial_n': nb % cn != 0, 'scalar': n % 8 != 0, 'tiles': tiles, 'stages': stages, 'kb': kb,
+            'multi_round': rounds > 1, 'kb_lt_stages': kb < stages, 'ring_repeats': kb % stages == 0}
 
 
 def _ragged_cases():
@@ -279,19 +311,24 @@ RAGGED_CASES = _ragged_cases()
 SCHEDULE_CASES = _schedule_cases()
 
 
-def query_plan(lib, case: GemmCase) -> dict:
-    """The plan geometry pe_debug_gemm_plan (host-only) reports for `case`, under the case's PE_GEMM_FORCE (if any)."""
+def query_geometry(lib, m, n, k, epi, force=None) -> dict:
+    """The plan geometry pe_debug_gemm_plan (host-only) reports for one shape, under PE_GEMM_FORCE = `force` (if any)."""
     out = (ctypes.c_int * 6)()
     old = os.environ.pop('PE_GEMM_FORCE', None)
     try:
-        if case.force:
-            os.environ['PE_GEMM_FORCE'] = case.force
-        lib.check(lib.LIB.pe_debug_gemm_plan(case.m, case.n, case.k, EPI[case.epi], out))
+        if force:
+            os.environ['PE_GEMM_FORCE'] = force
+        lib.check(lib.LIB.pe_debug_gemm_plan(m, n, k, EPI[epi], out))
     finally:
         os.environ.pop('PE_GEMM_FORCE', None)
         if old is not None:
             os.environ['PE_GEMM_FORCE'] = old
-    return plan_geometry(list(out), case.m, case.n)
+    return plan_geometry(list(out), m, n, k)
+
+
+def query_plan(lib, case) -> dict:
+    """The plan geometry of `case` (a GemmCase, or anything with m, n, k, epi, force), under its PE_GEMM_FORCE."""
+    return query_geometry(lib, case.m, case.n, case.k, case.epi, case.force)
 
 
 def expectation_failures(case: GemmCase, geom: dict):
@@ -316,7 +353,7 @@ def gemm_operands(case: GemmCase, seed: int):
 
 
 # ------------------------------------------------------------------------------------------------- attention
-ATTN_TOKENS = (1, 17, 31, 32, 33, 63, 64, 65, 197, 223, 225, 255, 256, 257, 300, 511, 512)
+ATTN_TOKENS = (1, 17, 31, 32, 33, 63, 64, 65, 128, 197, 198, 223, 225, 255, 256, 257, 300, 511, 512)
 ATTN_KINDS = ('mask', 'rescale_first', 'rescale_last', 'uniform', 'readout', 'large')
 
 
@@ -500,7 +537,7 @@ def linear_ln_ref(a16, w16, bias, resid, gamma, beta, eps, c=C_GEMM):
     takes that error as the LayerNorm's input error, plus the rounding of v itself. Returns (v, v_bound, ln, ln_bound)."""
     x, mag = gemm_ref(a16, w16, bias, resid)
     v = x + resid.double()
-    v_bound = c * U32 * mag
+    v_bound = gemm_bound(a16, w16, mag, c)
     ln, ln_bound = layernorm_ref(v, gamma, beta, eps, in_err=v_bound + U32 * v.abs())
     return v, v_bound, ln, ln_bound
 

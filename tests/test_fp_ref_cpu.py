@@ -100,6 +100,81 @@ def test_gelu_scan_covers_the_edges():
     assert bool((tiny > 0).any()) and bool((tiny < 0).any()) and bool((tiny.abs() < 1.2e-38).any())
 
 
+LONG_K_STAGES = 4     # ring depth of the stale-stage kernel: BN 160 / 224 plans run 4 stages
+
+
+def _kblock_gemm(a, w, bias, mutate=None, j=None):
+    """fp32 emulation of the wgmma main loop: k-blocks of 64 summed in fp32, in order, onto an fp32 accumulator, then
+    + bias. `mutate` plants one wrong k-block `j`: 'drop' (never added), 'twice' (added twice), 'stale' (the operands
+    of block j - LONG_K_STAGES, what a ring slot still holds when its refill was not waited for), 'f16' (the block's
+    64 products summed in fp16)."""
+    kb = a.shape[1] // 64
+    acc = torch.zeros(a.shape[0], w.shape[0])
+    for b in range(kb):
+        src = b - LONG_K_STAGES if (mutate == 'stale' and b == j) else b
+        sl = slice(64 * src, 64 * src + 64)
+        if mutate == 'f16' and b == j:
+            part = torch.zeros_like(acc).half()
+            for i in range(sl.start, sl.stop):   # fp16 x fp16 products are exact in fp32; the running sum is not
+                part = (part.float() + a[:, i, None].float() * w[None, :, i].float()).half()
+            blk = part.float()
+        else:
+            blk = a[:, sl].float() @ w[:, sl].float().t()
+        if not (mutate == 'drop' and b == j):
+            acc = acc + blk
+        if mutate == 'twice' and b == j:
+            acc = acc + blk
+    return acc + bias
+
+
+@pytest.mark.parametrize('k', [3072, 4096])
+def test_gemm_bound_at_long_k(k):
+    """At the K of the product's FC2 GEMMs (3072, 4096) the GEMM bound accepts an fp32 kernel that sums k-blocks of 64
+    in order, and rejects one wrong k-block out of 48 / 64: dropped, counted twice, taken from a stale ring slot, or
+    summed in fp16. Operands at model scale: A ~ N(0, 1), W ~ N(0, 0.03^2)."""
+    gen = torch.Generator().manual_seed(k)
+    m, n = 16, 24
+    a = torch.randn(m, k, generator=gen).half()
+    w = (torch.randn(n, k, generator=gen) * 0.03).half()
+    bias = torch.randn(n, generator=gen) * 0.05
+    right = _kblock_gemm(a, w, bias)
+    rep = R.check_gemm('F32', right, a, w, bias)
+    assert rep.passed, rep.describe(right, R.gemm_ref(a, w, bias, None)[0])
+    for j in (LONG_K_STAGES, k // 128, k // 64 - 1):
+        for mutate in ('drop', 'twice', 'stale', 'f16'):
+            wrong = _kblock_gemm(a, w, bias, mutate, j)
+            assert not R.check_gemm('F32', wrong, a, w, bias).passed, (mutate, j)
+
+
+def _truncating_gemm(a, w):
+    """An fp32 accumulator that adds each K_STEP products exactly and then rounds toward zero (the tensor cores'
+    accumulation, as far as the bound is concerned)."""
+    acc = torch.zeros(a.shape[0], w.shape[0], dtype=torch.float64)
+    for k0 in range(0, a.shape[1], R.K_STEP):
+        s = acc + a[:, k0:k0 + R.K_STEP].double() @ w[:, k0:k0 + R.K_STEP].double().t()   # exact: 16 products of fp16
+        f = s.float()
+        toward_zero = torch.nextafter(f, torch.zeros_like(f))
+        acc = torch.where(f.double().abs() > s.abs(), toward_zero, f).double()
+    return acc.float()
+
+
+def test_gemm_bound_covers_a_truncating_accumulator():
+    """Where every partial sum has the same sign (here: all operands positive) the truncation errors of the
+    accumulator add up with the number of k-steps: at K = 4096 they exceed C_GEMM u sum|a w|, the bound at K <= 776.
+    The partial-sum term of the bound (2 u per k-step) holds them, and the four wrong k-blocks stay rejected."""
+    gen = torch.Generator().manual_seed(5)
+    m, n, k = 16, 24, 4096
+    a = torch.rand(m, k, generator=gen).half()
+    w = (torch.rand(n, k, generator=gen) * 0.03).half()
+    got = _truncating_gemm(a, w)
+    x, mag = R.gemm_ref(a, w, None, None)
+    assert not R.check_f32(got, x, R.C_GEMM * R.U32 * mag).passed
+    rep = R.check_gemm('F32', got, a, w)
+    assert rep.passed, rep.describe(got, x)
+    for mutate in ('drop', 'twice', 'stale', 'f16'):
+        assert not R.check_gemm('F32', _kblock_gemm(a, w, 0.0, mutate, k // 128), a, w).passed, mutate
+
+
 # -------------------------------------------------------------------------------------------- attention checks
 def _attn(q, k, v):
     """fp64 attention of [B, H, S, d] tensors -> merged [B*S, H*d]."""

@@ -9,6 +9,7 @@ import json
 import os
 import subprocess
 import sys
+import zlib
 
 import pytest
 import torch
@@ -18,6 +19,7 @@ TESTS = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(TESTS)
 sys.path.insert(0, TESTS)
 import _fp_ref as R  # noqa: E402
+import _gemm_census as G  # noqa: E402
 
 gpu = pytest.mark.gpu
 pytestmark = gpu
@@ -121,6 +123,102 @@ def test_gemm_activation_scan(ops, n):
     t32 = ops.linear(a.cuda(), w.cuda(), b.cuda(), lib.PE_EPI_TANH_F32).cpu()
     _assert(R.check_gelu_scan(g16, x), g16, R.gelu64(x), 'gelu-scan')
     _assert(R.check_tanh_scan(t32, x), t32, torch.tanh(x), 'tanh-scan')
+
+
+PRODUCT_CASES = G.census(_lib())
+W_STD, BIAS_STD = 0.03, 0.05    # model-scale weights and biases (the synthetic checkpoints use 0.02)
+
+
+def _product_feeder(ops, case, k, gen):
+    """-> a function that launches the kernel that writes A [m, k] fp16 just before `case` in the product (on the
+    current stream, inputs already on the device) and returns A. The operands come out roughly N(0, 1), FC2's A is
+    the GELU output of an FC1 run as the stage runs it."""
+    m = case.m
+    if case.feeder == 'layernorm':
+        x = (torch.randn(m, k, generator=gen) * 1.5 + 0.3).cuda()
+        g = (1 + 0.1 * torch.randn(k, generator=gen)).cuda()
+        b = (0.1 * torch.randn(k, generator=gen)).cuda()
+        return lambda: ops.layernorm(x, g, b, 1e-6, want_f32=False, want_f16=True)[1]
+    if case.feeder == 'cast':
+        x = torch.randn(m, k, generator=gen).cuda()
+        a = torch.empty(m, k, dtype=torch.float16, device='cuda')
+        return lambda: (_cast(_lib().LIB.pe_cast_f32_to_f16, x, a, m * k), a)[1]
+    if case.feeder == 'attention':
+        spec = G.MODEL_SPECS[case.model]
+        qkv = torch.randn(m, 3 * k, generator=gen)
+        qkv[:, 2 * k:] *= (case.tokens / 3) ** 0.5       # the context (a weighted mean of V rows) comes out ~N(0, 1)
+        qkv = qkv.half().cuda()
+        return lambda: ops.attention(qkv, case.ub, case.tokens, spec.heads)
+    if case.feeder == 'fc1':
+        h = case.n                                        # FC2 [m, H] reads FC1's GELU output [m, I]
+        a0 = torch.randn(m, h, generator=gen).half().cuda()
+        w1 = (torch.randn(k, h, generator=gen) * W_STD).half().cuda()
+        b1 = (torch.randn(k, generator=gen) * BIAS_STD).cuda()
+        return lambda: ops.linear(a0, w1, b1, _lib().PE_EPI_GELU_F16, static_w=True)
+    raise ValueError(case.feeder)
+
+
+def _product_patch_embed(case, gen):
+    """The patch embedding as the first ViT / DeiT stage runs it (im2col, prefix rows, then the GEMM's row-remapped
+    RESID_F32 epilogue adding the position rows) -> (got [B * patches, H], A, W, bias, resid) for check_gemm."""
+    spec = G.MODEL_SPECS[case.model]
+    n_prefix = 2 if spec.family == 'deit' else 1
+    hidden, kpad, batch = case.n, case.k, case.ub
+    kdim = spec.channels * spec.patch ** 2
+    pixels = torch.randn(batch, spec.channels, spec.image_size, spec.image_size, generator=gen).cuda()
+    w16 = torch.zeros(hidden, kpad, dtype=torch.float16)
+    w16[:, :kdim] = (torch.randn(hidden, kdim, generator=gen) * W_STD).half()
+    w16 = w16.cuda()
+    bias = (torch.randn(hidden, generator=gen) * BIAS_STD).cuda()
+    pos = torch.randn(case.tokens, hidden, generator=gen).cuda()
+    prefix = torch.randn(n_prefix, hidden, generator=gen).cuda()
+    lib = _lib()
+    n_patches = case.tokens - n_prefix
+    out = torch.empty((batch, case.tokens, hidden), dtype=torch.float32, device='cuda')
+    work = torch.empty((batch * n_patches, kpad), dtype=torch.float16, device='cuda')
+    torch.cuda.synchronize()
+    lib.check(lib.LIB.pe_patch_embed(pixels.data_ptr(), w16.data_ptr(), bias.data_ptr(), pos.data_ptr(), prefix.data_ptr(),
+                                     out.data_ptr(), work.data_ptr(), batch, spec.channels, spec.image_size, spec.patch,
+                                     hidden, n_prefix, _stream()))
+    torch.cuda.synchronize()
+    assert torch.equal(out[:, :n_prefix], prefix.expand(batch, n_prefix, hidden))
+    resid = pos[n_prefix:].repeat(batch, 1)
+    return out[:, n_prefix:].reshape(batch * n_patches, hidden), work, w16, bias, resid
+
+
+@pytest.mark.parametrize('case', PRODUCT_CASES, ids=lambda c: c.name)
+def test_gemm_product_plans(ops, case):
+    """Every plan the supported models run (`_gemm_census`: one case per (epilogue, static_w, plan, ring depth, one
+    or several tiles per CTA, K loop against the ring, partly empty clusters, scalar epilogue), at its smallest
+    product shape, plus the benchmark's 16 GEMMs), run the way the product runs it: A written on the same stream, with
+    nothing synchronised in between, by the kernel that writes it in the product (LayerNorm, cast, attention, FC1's
+    GELU epilogue, im2col), stage GEMMs with static_w (W streamed before that kernel has finished), model-scale
+    operands. Every element against fp64 on the A actually produced."""
+    lib = _lib()
+    geom = R.query_plan(lib, case)
+    bad = R.expectation_failures(case, geom)
+    assert not bad, f"{case.name}: the planner no longer gives this call the plan of its census key: {bad}"
+    gen = torch.Generator().manual_seed(zlib.crc32(case.name.encode()))
+    if case.feeder == 'im2col':
+        got, a, w, bias, resid = _product_patch_embed(case, gen)
+    else:
+        w = (torch.randn(case.n, case.k, generator=gen) * W_STD).half().cuda()
+        bias = (torch.randn(case.n, generator=gen) * BIAS_STD).cuda()
+        resid = None
+        feed = _product_feeder(ops, case, case.k, gen)
+        torch.cuda.synchronize()
+        a = feed()
+        got = ops.linear(a, w, bias, R.EPI[case.epi], static_w=bool(case.static_w))
+        torch.cuda.synchronize()
+    rep = R.check_gemm(case.epi, got, a, w, bias, resid, where=case.name)
+    _record('gemm-product-' + case.epi, rep)
+    if case.k >= 3072:
+        _record('gemm-product-k>=3072-' + case.epi, rep)
+    if not rep.passed:
+        x, _ = R.gemm_ref(a, w, bias, None)
+        ref = {'RESID_F32': x + (0 if resid is None else resid.double()), 'TANH_F32': torch.tanh(x),
+               'GELU_F16': R.gelu64(x)}.get(case.epi, x)
+        pytest.fail(rep.describe(got, ref) + f"\n  plan {geom}")
 
 
 def test_gemm_dependent_chain_under_pdl(ops):
