@@ -2,29 +2,21 @@
 broadcast, FIFO ordering through a 2-stage pipeline with results returned to the data rank, tuple payloads,
 hooks. The reference's own lifecycle test (`test/comm/p2p/test_context.py:23-40`) is restated first."""
 import os
-import socket
+import sys
 import threading
 import torch
-import torch.multiprocessing as mp
 
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import _multirank as mr  # noqa: E402
 
-def _free_port() -> int:
-    with socket.socket() as s:
-        s.bind(('127.0.0.1', 0))
-        return s.getsockname()[1]
-
-
-def _env(port):
-    os.environ['MASTER_ADDR'] = '127.0.0.1'
-    os.environ['MASTER_PORT'] = str(port)
-    os.environ['CUDA_VISIBLE_DEVICES'] = ''   # this suite is the Gloo path
+ENV = {'CUDA_VISIBLE_DEVICES': ''}   # this suite is the Gloo path
 
 
 def test_context_lifecycle_world1(monkeypatch):
     from pipeedge_b200.comm.p2p import DistP2pContext
     # runs in the pytest process itself: hiding the GPU here (CUDA_VISIBLE_DEVICES) would hide it from every later test
     monkeypatch.setenv('MASTER_ADDR', '127.0.0.1')
-    monkeypatch.setenv('MASTER_PORT', str(_free_port()))
+    monkeypatch.setenv('MASTER_PORT', str(mr.free_port()))
     ctx = DistP2pContext(('gloo',), {'world_size': 1, 'rank': 0}, lambda cmd, tensors: None)
     ctx.init()
     ctx.shutdown()
@@ -32,8 +24,7 @@ def test_context_lifecycle_world1(monkeypatch):
         pass
 
 
-def _pipeline_worker(rank, world, port, n_ubatch, out_q):
-    _env(port)
+def _pipeline_worker(rank, world, n_ubatch):
     torch.set_num_threads(1)
     from pipeedge_b200.comm.p2p import DistP2pContext, DistP2pPipelineStage
     cmds = []
@@ -65,7 +56,7 @@ def _pipeline_worker(rank, world, port, n_ubatch, out_q):
                 assert done.wait(60), "results did not arrive"
                 stage.check_workers()
                 ctx.cmd_broadcast(0)   # as runtime.py: stop is broadcast before the stage context exits
-            out_q.put(('results', [r.tolist() for r in results], hook_log))
+            return [r.tolist() for r in results], hook_log
         else:
             def work(payload):
                 x, meta = payload
@@ -73,39 +64,26 @@ def _pipeline_worker(rank, world, port, n_ubatch, out_q):
                 return x * 2.0
             with DistP2pPipelineStage(0, 0, work, None):
                 assert stop.wait(60), "stop command did not arrive"
-            out_q.put(('cmds', cmds))
+            return cmds
 
 
 def test_two_rank_pipeline_fifo_and_commands():
-    ctx = mp.get_context('spawn')
-    out_q = ctx.Queue()
-    port = _free_port()
     n = 9
-    procs = [ctx.Process(target=_pipeline_worker, args=(r, 2, port, n, out_q)) for r in range(2)]
-    for p in procs:
-        p.start()
-    got = {}
-    for _ in range(2):
-        item = out_q.get(timeout=120)
-        got[item[0]] = item[1:]
-    for p in procs:
-        p.join(60)
-        assert p.exitcode == 0
-    results, hook_log = got['results']
+    got = mr.spawn(_pipeline_worker, 2, (n,), env=ENV, get_timeout=120, join_timeout=60)
+    results, hook_log = got[0]
     assert len(results) == n
     for i, r in enumerate(results):   # FIFO: result i is (i + 1) * 2 everywhere
         assert r == [[(i + 1) * 2.0] * 3] * 2
     assert hook_log == [('send', 2)] * n
-    (cmds,) = got['cmds']
+    cmds = got[1]
     assert cmds[0] == (1, [[[1, 4], [5, 8]], [0, 0], 7])
     assert cmds[-1][0] == 0
 
 
-def _ragged_worker(rank, world, port, out_q):
+def _ragged_worker(rank, world):
     """Payload layouts that change mid-stream: ragged last micro-batch, a tuple with constant host-side metadata, an
     empty tensor, dtype changes - the envelope protocol resends the full description only when the layout changes and
     hands out the SAME host tensors when their bytes did not change."""
-    _env(port)
     torch.set_num_threads(1)
     from pipeedge_b200.comm.p2p import DistP2pContext, DistP2pPipelineStage
     stop = threading.Event()
@@ -130,7 +108,7 @@ def _ragged_worker(rank, world, port, out_q):
                 assert done.wait(60), "results did not arrive"
                 stage.check_workers()
                 ctx.cmd_broadcast(0)
-            out_q.put(('results', [(str(r.dtype), list(r.shape), r.tolist()) for r in results]))
+            return [(str(r.dtype), list(r.shape), r.tolist()) for r in results]
         else:
             seen_meta = []
 
@@ -142,27 +120,15 @@ def _ragged_worker(rank, world, port, out_q):
             with DistP2pPipelineStage(0, 0, work, None):
                 assert stop.wait(60), "stop command did not arrive"
             # a payload made of the very same host tensors is not re-sent: the receiver hands out its objects again
-            out_q.put(('meta', len(seen_meta), sum(1 for a, b in zip(seen_meta, seen_meta[1:]) if a is b)))
+            return len(seen_meta), sum(1 for a, b in zip(seen_meta, seen_meta[1:]) if a is b)
 
 
 def test_ragged_and_changing_payload_layouts():
-    ctx = mp.get_context('spawn')
-    out_q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_ragged_worker, args=(r, 2, port, out_q)) for r in range(2)]
-    for p in procs:
-        p.start()
-    got = {}
-    for _ in range(2):
-        item = out_q.get(timeout=120)
-        got[item[0]] = item[1:]
-    for p in procs:
-        p.join(60)
-        assert p.exitcode == 0
-    (results,) = got['results']
+    got = mr.spawn(_ragged_worker, 2, env=ENV, get_timeout=120, join_timeout=60)
+    results = got[0]
     assert [r[1] for r in results] == [[4, 3], [4, 3], [2, 3], [0, 3], [2, 3], [4, 3]]
     assert results[0][2] == results[1][2] == [[2.0] * 3] * 4 and results[2][2] == [[6.0] * 3] * 2 and results[3][2] == []
     assert results[4][0] == 'torch.int64' and results[4][2] == [[0, 2, 4], [6, 8, 10]]
     assert results[5][0] == 'torch.float32' and results[5][2] == [[8.0] * 3] * 4
-    n_meta, n_same = got['meta']
+    n_meta, n_same = got[1]
     assert n_meta == 6 and n_same == 1      # payloads 0 and 1 were the same objects on the sender: received once

@@ -5,55 +5,22 @@ QuantPipe hooks run locally, the inputs the feeder takes, the kernel counts of b
 feeder and `runtime.py` with this topology. Ranks share one GPU (cudaIpc between processes of the same device), like
 `test_pipeline_gpu.py`."""
 import os
-import socket
-import subprocess
 import sys
 import numpy as np
 import pytest
 import torch
-import torch.multiprocessing as mp
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import _multirank as mr  # noqa: E402
 SEQ = 32   # BERT sequence length of every micro-batch
-
-
-def _free_port() -> int:
-    with socket.socket() as s:
-        s.bind(('127.0.0.1', 0))
-        return s.getsockname()[1]
-
-
-def _n_items(i, n_ubatch, ubatch):
-    return ubatch - 1 if i == n_ubatch - 1 else ubatch   # the last micro-batch is ragged
-
-
-def _make_shard(name, cuts, qbits, s, weights=None):
-    """Stage `s` of the pipeline cut after `cuts`, with the QuantPipe hooks `runtime.py` gives it."""
-    sys.path.insert(0, ROOT)
-    import runtime as rt
-    from pipeedge_b200.models import ModuleShardConfig
-    from pipeedge_b200.models.transformers import bert, deit, vit
-    from pipeedge_b200.synth import MODEL_SPECS, hf_config, synth_weights
-    spec = MODEL_SPECS[name]
-    classes = {'vit': vit.ViTShardForImageClassification, 'deit': deit.DeiTShardForImageClassification,
-               'bert': bert.BertShardForSequenceClassification}
-    lo = 1 if s == 0 else cuts[s - 1] + 1
-    cfg = ModuleShardConfig(layer_start=lo, layer_end=cuts[s], is_first=lo == 1, is_last=cuts[s] == spec.layers)
-    shard = classes[spec.family](hf_config(spec), cfg, weights if weights is not None else synth_weights(spec, seed=0))
-    shard.register_buffer('quant_bit', torch.tensor(qbits[s]), persistent=False)
-    if s != len(cuts) - 1:
-        shard.register_forward_hook(rt.forward_hook_quant_encode)
-    if s != 0:
-        shard.register_forward_pre_hook(rt.forward_pre_hook_quant_decode)
-    return shard
 
 
 def _input(spec, i, n_ubatch, ubatch, mixed):
     """Micro-batch i. `mixed`: a host tensor, a device tensor, or a host tensor of a dtype the feeder converts (float64
     images / int32 token ids, both converted exactly), in turn."""
     from pipeedge_b200.synth import synth_input
-    x = synth_input(spec, _n_items(i, n_ubatch, ubatch), seed=10 + i, seq_len=SEQ)
+    x = synth_input(spec, mr.ragged(i, n_ubatch, ubatch), seed=10 + i, seq_len=SEQ)
     if mixed and i % 3 == 1:
         return x.cuda()
     if mixed and i % 3 == 2:
@@ -65,7 +32,7 @@ def _inside_kernels(name, cuts, qbits, ubatch, dim1):
     """graph_kernels of the first stage when the data rank owns it (a world of one: host-fed input, loop-back output),
     for the full and the ragged micro-batch."""
     from pipeedge_b200.comm.p2p._native import NativeStage
-    stage = NativeStage(None, None, _make_shard(name, cuts, qbits, 0), lambda _t: None)
+    stage = NativeStage(None, None, mr.make_shard(name, cuts, 0, qbits[0]), lambda _t: None)
     stage.init(None, None)
     try:
         stage.prepare(ubatch, dim1)
@@ -75,24 +42,15 @@ def _inside_kernels(name, cuts, qbits, ubatch, dim1):
         stage.shutdown()
 
 
-def _worker(rank, world, port, name, cuts, qbits, n_ubatch, ubatch, mixed, hooked, out_q):
-    import faulthandler
+def _worker(rank, world, name, cuts, qbits, n_ubatch, ubatch, mixed, hooked):
     import threading
-    faulthandler.enable()   # a native crash prints every thread's Python stack into the test log
-    faulthandler.dump_traceback_later(300, exit=True)   # a hung rank shows where, and ends
-    sys.path.insert(0, ROOT)
-    os.environ.update(MASTER_ADDR='127.0.0.1', MASTER_PORT=str(port), PIPEEDGE_NATIVE='1')
-    os.environ.setdefault('PIPEEDGE_LINK_TIMEOUT_S', '60')   # ranks sharing one GPU are time-sliced
-    if mixed:
-        os.environ['PIPEEDGE_LINK_SLOTS'] = '2'   # the feeder outruns the first stage sooner: back-pressure
-    torch.cuda.set_device(rank % torch.cuda.device_count())
     import model_cfg
     from pipeedge_b200.comm.p2p import DistP2pContext
     from pipeedge_b200.synth import MODEL_SPECS
     spec = MODEL_SPECS[name]
     stage_ranks = list(range(1, world))
     s = rank - 1 if rank > 0 else None
-    shard = _make_shard(name, cuts, qbits, s) if s is not None else None
+    shard = mr.make_shard(name, cuts, s, qbits[s]) if s is not None else None
     stop = threading.Event()
     results, done, sends = [], threading.Event(), []
 
@@ -123,67 +81,30 @@ def _worker(rank, world, port, name, cuts, qbits, n_ubatch, ubatch, mixed, hooke
         out.update(results=results, sends=sends, geometry=native.input_geometry)
     if rank == 1:
         out['inside_kernels'] = _inside_kernels(name, cuts, qbits, ubatch, SEQ if spec.family == 'bert' else 0)
-    faulthandler.cancel_dump_traceback_later()
-    out_q.put((rank, out))
-    out_q.close()
-    out_q.join_thread()
+    return out
 
 
 def _run(name, cuts, qbits, n_ubatch, ubatch, mixed=False, hooked=False):
-    world = len(cuts) + 1
-    ctx = mp.get_context('spawn')
-    out_q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, name, cuts, qbits, n_ubatch, ubatch, mixed, hooked,
-                                               out_q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    got = {}
-    try:
-        for _ in range(world):
-            rank, out = out_q.get(timeout=600)
-            got[rank] = out
-    finally:
-        for p in procs:
-            p.join(180)
-            if p.is_alive():
-                p.kill()
-                p.join(10)
-    for r, p in enumerate(procs):
-        assert p.exitcode == 0, f"rank {r} exited with {p.exitcode}"
-    return got
-
-
-def _local_reference(name, cuts, qbits, n_ubatch, ubatch):
-    """The same shards + QuantPipe hooks back to back in this process."""
-    from pipeedge_b200.synth import MODEL_SPECS, synth_weights
-    spec = MODEL_SPECS[name]
-    weights = synth_weights(spec, seed=0)
-    shards = [_make_shard(name, cuts, qbits, s, weights) for s in range(len(cuts))]
-    outs = []
-    for i in range(n_ubatch):
-        x = _input(spec, i, n_ubatch, ubatch, False)
-        for shard in shards:
-            x = shard(x)
-        outs.append(x.cpu().numpy())
-    return outs
+    env = {'PIPEEDGE_NATIVE': '1'}
+    if mixed:
+        env['PIPEEDGE_LINK_SLOTS'] = '2'   # the feeder outruns the first stage sooner: back-pressure
+    return mr.spawn(_worker, len(cuts) + 1, (name, cuts, qbits, n_ubatch, ubatch, mixed, hooked), env=env,
+                    hang_dump=300)
 
 
 def _check(name, cuts, qbits, n_ubatch, ubatch, got):
-    from pipeedge_b200.synth import MODEL_SPECS, synth_weights
+    """Against the same shards + QuantPipe hooks back to back in this process."""
+    from pipeedge_b200.synth import MODEL_SPECS
+    spec = MODEL_SPECS[name]
+    inputs = [_input(spec, i, n_ubatch, ubatch, False) for i in range(n_ubatch)]
     results = got[0]['results']
     assert len(results) == n_ubatch
-    for i, (logits, want) in enumerate(zip(results, _local_reference(name, cuts, qbits, n_ubatch, ubatch))):
+    local = mr.run_local([mr.make_shard(name, cuts, s, qbits[s]) for s in range(len(cuts))], inputs)
+    for i, (logits, want) in enumerate(zip(results, local)):
         assert logits.shape == want.shape, i
         np.testing.assert_array_equal(logits, want, err_msg=f"micro-batch {i}")
     if not any(qbits):
-        sys.path.insert(0, ROOT)
-        from oracle import shards as osh
-        spec = MODEL_SPECS[name]
-        w = synth_weights(spec, seed=0)
-        for i, logits in enumerate(results):
-            want = osh.shard_forward(spec, w, 1, spec.layers, _input(spec, i, n_ubatch, ubatch, False)).numpy()
-            assert np.abs(logits - want).max() <= 4e-3 * np.abs(want).max(), f"micro-batch {i}"
+        mr.assert_within_oracle(name, results, inputs)
 
 
 def _shapes(name, ubatch):
@@ -241,24 +162,19 @@ def test_relay_capture_refuses_oversized_inputs_before_launching():
     import ctypes
     from pipeedge_b200._lib import LIB, PipeEdgeB200Error, check
     torch.cuda.set_device(0)
-    link_in, loop, pipe, other = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_void_p()
+    other = ctypes.c_void_p()
     kernels = ctypes.c_int()
-    check(LIB.pe_link_open_host(4096, 2, ctypes.byref(link_in)))
-    check(LIB.pe_link_open_local(4096, 2, 0, ctypes.byref(loop)))
-    try:
-        check(LIB.pe_pipe_create(link_in, loop, loop, ctypes.byref(pipe)))
-        room = LIB.pe_link_slot_bytes(link_in)
-        with pytest.raises(PipeEdgeB200Error, match='exceed'):
-            check(LIB.pe_pipe_capture_relay(pipe, 1, 0, room + 1, ctypes.byref(kernels)))
-        assert LIB.pe_pipe_has_graph(pipe, 1, 0) == 0
-        check(LIB.pe_pipe_create(loop, loop, None, ctypes.byref(other)))
-        with pytest.raises(PipeEdgeB200Error, match='not host-fed'):
-            check(LIB.pe_pipe_capture_relay(other, 1, 0, 64, ctypes.byref(kernels)))
-    finally:
-        LIB.pe_pipe_destroy(other)
-        LIB.pe_pipe_destroy(pipe)
-        LIB.pe_link_close(loop)
-        LIB.pe_link_close(link_in)
+    with mr.LoopbackPipe(4096, 4096, slots=2) as lp:
+        try:
+            room = LIB.pe_link_slot_bytes(lp.link_in)
+            with pytest.raises(PipeEdgeB200Error, match='exceed'):
+                check(LIB.pe_pipe_capture_relay(lp.pipe, 1, 0, room + 1, ctypes.byref(kernels)))
+            assert LIB.pe_pipe_has_graph(lp.pipe, 1, 0) == 0
+            check(LIB.pe_pipe_create(lp.loop, lp.loop, None, ctypes.byref(other)))
+            with pytest.raises(PipeEdgeB200Error, match='not host-fed'):
+                check(LIB.pe_pipe_capture_relay(other, 1, 0, 64, ctypes.byref(kernels)))
+        finally:
+            LIB.pe_pipe_destroy(other)
 
 
 def test_relay_moves_the_bytes_unchanged_through_a_loop_back_link():
@@ -268,12 +184,9 @@ def test_relay_moves_the_bytes_unchanged_through_a_loop_back_link():
     import ctypes
     from pipeedge_b200._lib import LIB, check
     torch.cuda.set_device(0)
-    link_in, loop, pipe = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_void_p()
-    check(LIB.pe_link_open_host(1 << 20, 2, ctypes.byref(link_in)))
-    check(LIB.pe_link_open_local(1 << 20, 2, 0, ctypes.byref(loop)))
     kernels = ctypes.c_int()
-    try:
-        check(LIB.pe_pipe_create(link_in, loop, None, ctypes.byref(pipe)))
+    with mr.LoopbackPipe(1 << 20, 1 << 20, slots=2, results=False) as lp:
+        pipe, loop = lp.pipe, lp.loop
         gen = torch.Generator().manual_seed(7)
         srcs = [torch.randn(3, 3, 64, 64, generator=gen), torch.randint(-2**62, 2**62, (5, 32), generator=gen),
                 torch.randn(1, 37, generator=gen), torch.randn(3, 3, 64, 64, generator=gen)]
@@ -290,10 +203,6 @@ def test_relay_moves_the_bytes_unchanged_through_a_loop_back_link():
             assert torch.equal(buf[:nbytes].cpu(), src.view(-1).view(torch.uint8))
         check(LIB.pe_pipe_sync(pipe))
         assert LIB.pe_link_check(loop) == 0
-    finally:
-        LIB.pe_pipe_destroy(pipe)
-        LIB.pe_link_close(loop)
-        LIB.pe_link_close(link_in)
 
 
 def _raw_receive(link, buf, nbytes, items):
@@ -333,29 +242,10 @@ def test_runtime_with_the_data_rank_outside(env, expect, tmp_path):
     heartbeats; with a send-rate constraint no hop can meet, the controller on the first stage's rank moves the
     bit-width off 'no quantization'."""
     import re
-    port = _free_port()
     base = dict(os.environ, PYTHONUNBUFFERED='1', PIPEEDGE_LINK_TIMEOUT_S='60', MONITORING='0')
     base.update(env)
-    cmd = [sys.executable, os.path.join(ROOT, 'runtime.py'), None, '3', '--port', str(port), '-m',
-           'facebook/deit-tiny-distilled-patch16-224', '-b', '64', '-u', '8', '-pt', '1,24,25,48', '-q', '0,0',
-           '-r', '1,2', '-D', '0']
-    procs = []
-    for rank in (2, 1, 0):
-        argv = list(cmd)
-        argv[2] = str(rank)
-        procs.append(subprocess.Popen(argv, cwd=str(tmp_path), env=dict(base, LOCAL_RANK=str(rank)),
-                                      stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True))
-    outs = []
-    for p in procs:
-        try:
-            out, _ = p.communicate(timeout=600)
-        except subprocess.TimeoutExpired:
-            p.kill()
-            out, _ = p.communicate()
-        outs.append(out)
-    for p, out in zip(procs, outs):
-        assert p.returncode == 0, out[-3000:]
-    rank2, rank1, rank0 = outs
+    outs = mr.run_runtime(tmp_path, 3, ['-q', '0,0', '-r', '1,2', '-D', '0'], base)
+    rank2, rank1, rank0 = outs[2], outs[1], outs[0]
     assert 'Data rank: native' in rank0, rank0[-3000:]
     assert 'throughput is' in rank0, rank0[-3000:]
     for out in (rank1, rank2):

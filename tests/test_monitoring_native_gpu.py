@@ -3,15 +3,14 @@ and the send-timing hook fed from them. Multi-rank pipelines share one GPU (cuda
 device), like `test_pipeline_gpu.py`."""
 import ctypes
 import os
-import socket
 import sys
 import numpy as np
 import pytest
 import torch
-import torch.multiprocessing as mp
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import _multirank as mr  # noqa: E402
 KEYS = ('shard', 'quant_encode', 'quant_decode', 'send')
 # stamp kernels per micro-batch: Start, Got, Stage(+SendStart), SendEnd with the send in the main graph; a separate
 # SendStart in the send graph when it overlaps; one more (Encoded) on a staged send
@@ -21,47 +20,13 @@ STAMPS_IN_GRAPH, STAMPS_OVERLAPPED, STAMPS_STAGED = 4, 5, 1
 SLACK_MS = 0.1
 
 
-def _free_port() -> int:
-    with socket.socket() as s:
-        s.bind(('127.0.0.1', 0))
-        return s.getsockname()[1]
-
-
-def _shard(spec, rank, cuts, qbits, world, rt, extra_hooks=()):
-    from pipeedge_b200.models import ModuleShardConfig
-    from pipeedge_b200.models.transformers import deit, vit
-    from pipeedge_b200.synth import hf_config, synth_weights
-    classes = {'vit': vit.ViTShardForImageClassification, 'deit': deit.DeiTShardForImageClassification}
-    lo = 1 if rank == 0 else cuts[rank - 1] + 1
-    cfg = ModuleShardConfig(layer_start=lo, layer_end=cuts[rank], is_first=lo == 1, is_last=cuts[rank] == spec.layers)
-    shard = classes[spec.family](hf_config(spec), cfg, synth_weights(spec, seed=0))
-    shard.register_buffer('quant_bit', torch.tensor(qbits[rank]), persistent=False)
-    for hook in extra_hooks:
-        shard.register_forward_hook(hook)
-    shard.register_forward_hook(rt.forward_hook_monitor)
-    if rank != world - 1:
-        shard.register_forward_hook(rt.forward_hook_quant_encode)
-    if rank != 0:
-        shard.register_forward_pre_hook(rt.forward_pre_hook_quant_decode)
-    shard.register_forward_pre_hook(rt.forward_pre_hook_monitor)
-    return shard
-
-
 def _inputs(spec, n_ubatch, ubatch):
     from pipeedge_b200.synth import synth_input
-    return [synth_input(spec, ubatch - 1 if i == n_ubatch - 1 else ubatch, seed=10 + i) for i in range(n_ubatch)]
+    return [synth_input(spec, mr.ragged(i, n_ubatch, ubatch), seed=10 + i) for i in range(n_ubatch)]
 
 
-def _worker(rank, world, port, name, cuts, qbits, n_ubatch, ubatch, overlap, out_q):
-    import faulthandler
+def _worker(rank, world, name, cuts, qbits, n_ubatch, ubatch):
     import threading
-    faulthandler.enable()
-    faulthandler.dump_traceback_later(300, exit=True)
-    sys.path.insert(0, ROOT)
-    os.environ.update(MASTER_ADDR='127.0.0.1', MASTER_PORT=str(port), PIPEEDGE_NATIVE='1',
-                      PIPEEDGE_OVERLAP_SEND=str(overlap))
-    os.environ.setdefault('PIPEEDGE_LINK_TIMEOUT_S', '60')
-    torch.cuda.set_device(rank % torch.cuda.device_count())
     import monitoring
     import runtime as rt
     from pipeedge_b200.comm.p2p import DistP2pContext, DistP2pPipelineStage
@@ -76,7 +41,7 @@ def _worker(rank, world, port, name, cuts, qbits, n_ubatch, ubatch, overlap, out
         marker = lambda *_: None   # noqa: E731  (a no-op hook that collects the stage's records)
         marker._pe_native = True
         marker._pe_records = lambda _shard: records.append
-        shard = _shard(spec, rank, cuts, qbits, world, rt, extra_hooks=(marker,) if monitored else ())
+        shard = mr.make_shard(name, cuts, rank, qbits[rank], hooks=(marker,) if monitored else (), monitor=True)
         results, done = [], threading.Event()
 
         def results_cb(t):
@@ -117,17 +82,12 @@ def _worker(rank, world, port, name, cuts, qbits, n_ubatch, ubatch, overlap, out
         with monitoring.get_locked_context(rt.MONITORING_KEY_SEND) as mctx:
             on['tags'] = {k: mctx.get_tag(key=k) for k in KEYS}
         monitoring.finish()
-    faulthandler.cancel_dump_traceback_later()
-    out_q.put((rank, off, on))
-    out_q.close()
-    out_q.join_thread()
+    return off, on
 
 
 def _local(name, cuts, qbits, n_ubatch, ubatch):
     """The same shards + QuantPipe hooks back to back in this process; also the bytes the thread path would send per
     stage and micro-batch (its CUDA tensors: the activation, or codes + scale + shift)."""
-    sys.path.insert(0, ROOT)
-    import runtime as rt
     from pipeedge_b200 import _lib
     from pipeedge_b200.synth import MODEL_SPECS
     spec = MODEL_SPECS[name]
@@ -142,38 +102,13 @@ def _local(name, cuts, qbits, n_ubatch, ubatch):
                                for t in outs))
         return hook
 
-    shards = [_shard(spec, r, cuts, qbits, world, rt, extra_hooks=(sizer(r),)) for r in range(world)]
-    logits = []
-    for x in _inputs(spec, n_ubatch, ubatch):
-        for shard in shards:
-            x = shard(x)
-        logits.append(x.cpu().numpy())
-    return logits, sent
+    shards = [mr.make_shard(name, cuts, r, qbits[r], hooks=(sizer(r),), monitor=True) for r in range(world)]
+    return mr.run_local(shards, _inputs(spec, n_ubatch, ubatch)), sent
 
 
 def _run(name, cuts, qbits, n_ubatch, ubatch, overlap):
-    world = len(cuts)
-    ctx = mp.get_context('spawn')
-    out_q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, name, cuts, qbits, n_ubatch, ubatch, overlap, out_q))
-             for r in range(world)]
-    for p in procs:
-        p.start()
-    got = {}
-    try:
-        for _ in range(world):
-            rank, off, on = out_q.get(timeout=600)
-            got[rank] = (off, on)
-    finally:
-        for p in procs:
-            p.join(180)
-            if p.is_alive():
-                p.kill()
-                p.join(10)
-    for r, p in enumerate(procs):
-        assert p.exitcode == 0, f"rank {r} exited with {p.exitcode}"
-    return got
+    env = {'PIPEEDGE_NATIVE': '1', 'PIPEEDGE_OVERLAP_SEND': str(overlap)}
+    return mr.spawn(_worker, len(cuts), (name, cuts, qbits, n_ubatch, ubatch), env=env, hang_dump=300)
 
 
 @pytest.mark.parametrize('overlap', [1, 0])
@@ -249,33 +184,17 @@ def test_stamp_ring_recapture_and_dropped_records():
     torch.cuda.set_device(0)
     items, n = 2, 256
     nbytes = items * n * 4
-    link_in, loop, pipe = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_void_p()
-    check(LIB.pe_link_open_host(nbytes, 4, ctypes.byref(link_in)))
-    check(LIB.pe_link_open_local(nbytes, 4, 0, ctypes.byref(loop)))
-    check(LIB.pe_pipe_create(link_in, loop, loop, ctypes.byref(pipe)))
-    buf = torch.zeros(items * n, dtype=torch.float32, device='cuda')
     src = torch.arange(items * n, dtype=torch.float32).pin_memory()
-    try:
-        check(LIB.pe_pipe_set_out_dim(pipe, n))
-
-        def capture():
-            kernels = ctypes.c_int()
-            check(LIB.pe_pipe_capture_begin(pipe, items, 0, 0, buf.data_ptr(), None, 0, 0, nbytes))
-            check(LIB.pe_pipe_capture_end(pipe, buf.data_ptr(), None, n, None, None, 0, items, 0, 0, 0,
-                                          ctypes.byref(kernels)))
-            return kernels.value
-
-        plain = capture()
+    with mr.LoopbackPipe(nbytes, nbytes) as lp:
+        pipe = lp.pipe
+        plain = lp.capture(items, n, 0, nbytes)
         assert LIB.pe_pipe_has_graph(pipe, items, 0) == 1
         check(LIB.pe_pipe_enable_stamps(pipe, 1))
         assert LIB.pe_pipe_has_graph(pipe, items, 0) == 0
-        assert capture() == plain + STAMPS_IN_GRAPH
+        assert lp.capture(items, n, 0, nbytes) == plain + STAMPS_IN_GRAPH
         depth, total = _lib.PE_PIPE_STAMP_DEPTH, _lib.PE_PIPE_STAMP_DEPTH + 44
-        ptr, got_items, got_n = ctypes.c_void_p(), ctypes.c_int(), ctypes.c_size_t()
         for _ in range(total):
-            check(LIB.pe_pipe_submit(pipe, src.data_ptr(), nbytes, 1, items, 0))
-            check(LIB.pe_pipe_next_result(pipe, ctypes.byref(ptr), ctypes.byref(got_items), ctypes.byref(got_n)))
-            out = np.ctypeslib.as_array(ctypes.cast(ptr, ctypes.POINTER(ctypes.c_float)), shape=(items * n,))
+            out = lp.submit_and_drain(src, items, n)
             assert np.array_equal(out, src.numpy())
         check(LIB.pe_pipe_sync(pipe))
         recs = (_lib.PipeRecord * (2 * depth))()
@@ -292,39 +211,16 @@ def test_stamp_ring_recapture_and_dropped_records():
         # stamps off again: the stamped graph counts as missing, and the plain capture is what it was
         check(LIB.pe_pipe_enable_stamps(pipe, 0))
         assert LIB.pe_pipe_has_graph(pipe, items, 0) == 0
-        assert capture() == plain
-    finally:
-        LIB.pe_pipe_destroy(pipe)
-        LIB.pe_link_close(loop)
-        LIB.pe_link_close(link_in)
+        assert lp.capture(items, n, 0, nbytes) == plain
 
 
 def test_runtime_monitoring_on_the_native_pipeline(tmp_path):
     """`runtime.py` on 2 ranks sharing one GPU with MONITORING=1 and no adaptive policy: it runs on the native pipeline
     and prints the monitored keys' global figures."""
-    import subprocess
-    port = _free_port()
     env = dict(os.environ, MONITORING='1', PYTHONUNBUFFERED='1', PIPEEDGE_LINK_TIMEOUT_S='60')
     env.pop('ADAPTIVE_QUANT', None)
-    cmd = [sys.executable, os.path.join(ROOT, 'runtime.py'), None, '2', '--port', str(port), '-m',
-           'facebook/deit-tiny-distilled-patch16-224', '-b', '64', '-u', '8', '-pt', '1,24,25,48', '-q', '8,0']
-    procs = []
-    for rank in (1, 0):
-        argv = list(cmd)
-        argv[2] = str(rank)
-        procs.append(subprocess.Popen(argv, cwd=str(tmp_path), env=dict(env, LOCAL_RANK=str(rank)), stdout=subprocess.PIPE,
-                                      stderr=subprocess.STDOUT, text=True))
-    outs = []
-    for p in procs:
-        try:
-            out, _ = p.communicate(timeout=600)
-        except subprocess.TimeoutExpired:
-            p.kill()
-            out, _ = p.communicate()
-        outs.append(out)
-    for p, out in zip(procs, outs):
-        assert p.returncode == 0, out[-3000:]
-    rank1, rank0 = outs
+    outs = mr.run_runtime(tmp_path, 2, ['-q', '8,0'], env)
+    rank1, rank0 = outs[1], outs[0]
     assert 'throughput is' in rank0, rank0[-3000:]
     for out in (rank0, rank1):
         assert 'Pipeline stage: native' in out, out[-3000:]

@@ -4,51 +4,28 @@ the CPU oracle. The native pipeline (peer-memory links, `comm/p2p/_native.py`) a
 (cudaIpc between processes of the same device), so these tests do not need a multi-GPU box; the NCCL / Python-thread
 path (`PIPEEDGE_NATIVE=0`) needs one GPU per rank and is skipped otherwise."""
 import os
-import socket
+import sys
+import numpy as np
 import pytest
 import torch
-import torch.multiprocessing as mp
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import _multirank as mr  # noqa: E402
 
 
-def _free_port() -> int:
-    with socket.socket() as s:
-        s.bind(('127.0.0.1', 0))
-        return s.getsockname()[1]
+def _inputs(name, n_ubatch, ubatch):
+    from pipeedge_b200.synth import MODEL_SPECS, synth_input
+    return [synth_input(MODEL_SPECS[name], mr.ragged(i, n_ubatch, ubatch), seed=10 + i, seq_len=32)
+            for i in range(n_ubatch)]
 
 
-def _worker(rank, world, port, name, cuts, qbits, n_ubatch, ubatch, out_q, native=True):
-    import faulthandler
-    import sys
+def _worker(rank, world, name, cuts, qbits, n_ubatch, ubatch, native):
     import threading
-    faulthandler.enable()   # a native crash prints every thread's Python stack into the test log
-    faulthandler.dump_traceback_later(240, exit=True)   # a hung rank shows where, and ends (instead of the whole test run)
-    sys.path.insert(0, ROOT)
-    os.environ['MASTER_ADDR'] = '127.0.0.1'
-    os.environ['MASTER_PORT'] = str(port)
-    os.environ['PIPEEDGE_NATIVE'] = '1' if native else '0'
-    os.environ.setdefault('PIPEEDGE_LINK_TIMEOUT_S', '60')   # ranks sharing one GPU are time-sliced
-    torch.cuda.set_device(rank % torch.cuda.device_count())
-    import runtime as rt
     from pipeedge_b200.comm.p2p import DistP2pContext, DistP2pPipelineStage
-    from pipeedge_b200.models import ModuleShardConfig
-    from pipeedge_b200.models.transformers import bert, deit, vit
-    from pipeedge_b200.synth import MODEL_SPECS, hf_config, synth_input, synth_weights
-    spec = MODEL_SPECS[name]
-    classes = {'vit': vit.ViTShardForImageClassification, 'deit': deit.DeiTShardForImageClassification,
-               'bert': bert.BertShardForSequenceClassification}
-    lo = 1 if rank == 0 else cuts[rank - 1] + 1
-    hi = cuts[rank]
-    cfg = ModuleShardConfig(layer_start=lo, layer_end=hi, is_first=lo == 1, is_last=hi == spec.layers)
-    shard = classes[spec.family](hf_config(spec), cfg, synth_weights(spec, seed=0))
+    shard = mr.make_shard(name, cuts, rank, qbits[rank])
     shard.use_cuda_graph = True
-    shard.register_buffer('quant_bit', torch.tensor(qbits[rank]), persistent=False)
-    if rank != world - 1:
-        shard.register_forward_hook(rt.forward_hook_quant_encode)
-    if rank != 0:
-        shard.register_forward_pre_hook(rt.forward_pre_hook_quant_decode)
     stop = threading.Event()
     results = []
     done = threading.Event()
@@ -64,99 +41,37 @@ def _worker(rank, world, port, name, cuts, qbits, n_ubatch, ubatch, out_q, nativ
         with DistP2pPipelineStage(src, dst, shard, results_cb if rank == 0 else None) as stage:
             assert (stage.native is not None) == native, "unexpected pipeline implementation"
             if rank == 0:
-                for i in range(n_ubatch):
-                    # the last micro-batch is ragged (one item short): a second graph is captured mid-stream
-                    n_items = ubatch - 1 if (i == n_ubatch - 1 and ubatch > 1) else ubatch
-                    stage.enqueue_tensor(synth_input(spec, n_items, seed=10 + i, seq_len=32))
+                # the last micro-batch is ragged (one item short): a second graph is captured mid-stream
+                for x in _inputs(name, n_ubatch, ubatch):
+                    stage.enqueue_tensor(x)
                 assert done.wait(300), "results did not arrive"
                 stage.check_workers()
                 ctx.cmd_broadcast(0)
-                out_q.put([r.numpy() for r in results])
             else:
                 assert stop.wait(420)
                 stage.check_workers()
-    faulthandler.cancel_dump_traceback_later()
-    out_q.close()
-    out_q.join_thread()
-    sys.stdout.flush()
-    sys.stderr.flush()
-    if not native:
-        # NCCL path: leave without the exit-time teardown of the CUDA / NCCL libraries (it can crash after a clean
-        # shutdown). The native pipeline owns no communicator and exits normally.
-        os._exit(0)
-
-
-def _local_reference(name, cuts, qbits, n_ubatch, ubatch):
-    """The same shards + QuantPipe hooks run back to back in THIS process on cuda:0 (no communication)."""
-    import sys
-    sys.path.insert(0, ROOT)
-    import runtime as rt
-    from pipeedge_b200.models import ModuleShardConfig
-    from pipeedge_b200.models.transformers import bert, deit, vit
-    from pipeedge_b200.synth import MODEL_SPECS, hf_config, synth_input, synth_weights
-    spec = MODEL_SPECS[name]
-    classes = {'vit': vit.ViTShardForImageClassification, 'deit': deit.DeiTShardForImageClassification,
-               'bert': bert.BertShardForSequenceClassification}
-    weights = synth_weights(spec, seed=0)
-    shards = []
-    for rank in range(len(cuts)):
-        lo = 1 if rank == 0 else cuts[rank - 1] + 1
-        cfg = ModuleShardConfig(layer_start=lo, layer_end=cuts[rank], is_first=lo == 1, is_last=cuts[rank] == spec.layers)
-        shard = classes[spec.family](hf_config(spec), cfg, weights)
-        shard.register_buffer('quant_bit', torch.tensor(qbits[rank]), persistent=False)
-        shards.append(shard)
-    for shard in shards[:-1]:
-        shard.register_forward_hook(rt.forward_hook_quant_encode)
-    for shard in shards[1:]:
-        shard.register_forward_pre_hook(rt.forward_pre_hook_quant_decode)
-    outs = []
-    for i in range(n_ubatch):
-        n_items = ubatch - 1 if (i == n_ubatch - 1 and ubatch > 1) else ubatch
-        data = synth_input(spec, n_items, seed=10 + i, seq_len=32)
-        for shard in shards:
-            data = shard(data)
-        outs.append(data.cpu().numpy())
-    return outs
+    return [r.numpy() for r in results] if rank == 0 else None
 
 
 def _run_pipeline(name, cuts, qbits, n_ubatch, ubatch, native):
-    world = len(cuts)
-    ctx = mp.get_context('spawn')
-    out_q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, name, cuts, qbits, n_ubatch, ubatch, out_q, native))
-             for r in range(world)]
-    for p in procs:
-        p.start()
-    try:
-        got = out_q.get(timeout=300)   # a fresh box pages torch in for a minute per process
-    finally:
-        for r, p in enumerate(procs):
-            p.join(180)
-            if p.is_alive():
-                p.kill()
-                p.join(10)
-    for r, p in enumerate(procs):
-        assert p.exitcode == 0, f"rank {r} exited with {p.exitcode}"
-    return got
+    # NCCL path: the ranks leave without the exit-time teardown of the CUDA / NCCL libraries (it can crash after a clean
+    # shutdown). The native pipeline owns no communicator and exits normally.
+    got = mr.spawn(_worker, len(cuts), (name, cuts, qbits, n_ubatch, ubatch, native),
+                   env={'PIPEEDGE_NATIVE': '1' if native else '0'},
+                   get_timeout=300,   # a fresh box pages torch in for a minute per process
+                   hang_dump=240, hard_exit=not native)
+    return got[0]
 
 
 def _check_against_local_and_oracle(name, cuts, qbits, n_ubatch, ubatch, got):
-    import numpy as np
-    from oracle import shards as osh
-    from pipeedge_b200.synth import MODEL_SPECS, synth_input, synth_weights
+    """Against the same shards + QuantPipe hooks run back to back in THIS process on cuda:0 (no communication)."""
     assert len(got) == n_ubatch
-    local = _local_reference(name, cuts, qbits, n_ubatch, ubatch)
+    inputs = _inputs(name, n_ubatch, ubatch)
+    local = mr.run_local([mr.make_shard(name, cuts, s, qbits[s]) for s in range(len(cuts))], inputs)
     for i, (logits, want) in enumerate(zip(got, local)):
         np.testing.assert_array_equal(logits, want, err_msg=f"micro-batch {i}")
     if not any(qbits):
-        spec = MODEL_SPECS[name]
-        w = synth_weights(spec, seed=0)
-        for i, logits in enumerate(got):
-            n_items = ubatch - 1 if (i == n_ubatch - 1 and ubatch > 1) else ubatch
-            x = synth_input(spec, n_items, seed=10 + i, seq_len=32)
-            want = osh.shard_forward(spec, w, 1, spec.layers, x).numpy()
-            assert np.abs(logits - want).max() <= 4e-3 * np.abs(want).max(), f"ubatch {i}"
+        mr.assert_within_oracle(name, got, inputs)
 
 
 @pytest.mark.parametrize('name,cuts,qbits', [
@@ -230,30 +145,9 @@ def test_runtime_cli_adaptive_quant(policy, tmp_path):
     must still deliver every result (`runtime.py:121-216,465-477` of the reference)."""
     if not torch.cuda.is_available() or torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs")
-    import subprocess
-    import sys
-    port = _free_port()
     env = dict(os.environ, ADAPTIVE_QUANT=policy, SEND_CONSTRAINT='1e9', WINDOW_SIZE='2', PYTHONUNBUFFERED='1',
                MONITORING='1' if policy == 'CONTROLLER' else '0')   # one run also with the opt-in device-timed heartbeats
-    cmd = [sys.executable, os.path.join(ROOT, 'runtime.py'), None, '2', '--port', str(port), '-m',
-           'facebook/deit-tiny-distilled-patch16-224', '-b', '64', '-u', '8', '-pt', '1,24,25,48', '-q', '0,0']
-    procs = []
-    for rank in (1, 0):
-        argv = list(cmd)
-        argv[2] = str(rank)
-        procs.append(subprocess.Popen(argv, cwd=str(tmp_path), env=dict(env, LOCAL_RANK=str(rank)), stdout=subprocess.PIPE,
-                                      stderr=subprocess.STDOUT, text=True))
-    outs = []
-    for p in procs:
-        try:
-            out, _ = p.communicate(timeout=600)
-        except subprocess.TimeoutExpired:
-            p.kill()
-            out, _ = p.communicate()
-        outs.append(out)
-    for p, out in zip(procs, outs):
-        assert p.returncode == 0, out[-3000:]
-    rank0 = outs[1]
+    rank0 = mr.run_runtime(tmp_path, 2, ['-q', '0,0'], env)[0]
     assert 'throughput is' in rank0, rank0[-3000:]
     import re
     bits = [int(b) for b in re.findall(r'Adaptive quantization \(\w+\): bitwidth1?=(\d+)', rank0)]
