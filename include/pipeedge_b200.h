@@ -363,7 +363,8 @@ int pe_debug_linear_simt(const void* a, const void* w, const void* bias, const v
 
 /* While `buf` (device, >= 32 * 8 * grid bytes) is set, every pe_linear launch stores a per-CTA clock64 timeline
  * (start, setup done, first operands landed, last MMA issued, accumulator ready, epilogue done, exit, epilogue and
- * steady-state main-loop detail; 32 slots per CTA). */
+ * steady-state main-loop detail; 32 slots per CTA). Slots 2, 3 and 5 (first operands landed, last MMA retired, epilogue
+ * done) are stamped for a CTA's first tile, slots 7, 8 and 10 the same for its second (scripts/gemm_phases.py). */
 int pe_debug_gemm_trace(void* buf);
 
 /* Host-only (no device needed): the tile plan and launch geometry pe_linear would use for an [m, k] x [n, k]^T product

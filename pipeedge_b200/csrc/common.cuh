@@ -260,6 +260,10 @@ template <int kId>
 __device__ __forceinline__ void named_barrier(int threads) {
   asm volatile("bar.sync %0, %1;" ::"n"(kId), "r"(threads) : "memory");
 }
+// the same with a barrier id known only at run time (e.g. one per warpgroup)
+__device__ __forceinline__ void named_barrier_id(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
 
 // ---------------------------------------------------------------- wgmma (warpgroup MMA)
 // Order this thread's earlier register / shared-memory accesses before the wgmma instructions that follow.

@@ -6,8 +6,12 @@
 //   warp 9      TMA producer for the weights: boxes of W [BN x 64] into the same stages
 //   warps 0..7  two consumer warpgroups: warpgroup g issues wgmma.mma_async (M=64, N=BN, K=16) x4 per stage on rows
 //               [64g, 64g+64) of the tile, accumulating fp32 in registers; once a stage's wgmmas have retired
-//               (wgmma.wait_group) it is released to its writers (`empty`). After the last K block every warp applies
-//               the epilogue to its 16 x BN slice of the accumulator (bias / GELU / residual / LayerNorm) and stores it.
+//               (wgmma.wait_group) it is released to its writers (`empty`). After the last K block each warpgroup
+//               applies the epilogue (bias / GELU / tanh / residual) to its accumulator fragments in registers, writes
+//               the results into its half of the staging area in the TMA swizzle and one thread stores the 64 x BN
+//               half tile with cp.async.bulk.tensor; the warpgroup goes straight on to its next tile and waits for
+//               those stores to have READ the staging only before it writes the staging again. The row-remap
+//               (patch embedding) and LayerNorm epilogues, and outputs TMA cannot address, store from registers.
 // While the consumers run an epilogue the producers already fill the ring with the next tile's operands.
 //
 // CTAs may be launched as thread-block CLUSTERS of CM x CN: the CM CTAs that share a W tile each load 1/CM of it and
@@ -64,6 +68,7 @@ struct GemmParams {
   int resid_per_item;  // 1: resid is [out_item_rows, n] shared by all items
   int stg_offset;      // byte offset of the epilogue staging from the ring base: 0 = aliases the ring (one tile per CTA)
   int static_w;        // 1: W is not written by anything still pending on the stream -> may be read before pdl_wait()
+  int tma_out;         // 1: the epilogue stores through the output tensor map (epilogue_tma), 0: from registers
   // PE_EPI_RESID_LN: v = A W^T + bias + resid, then LayerNorm(v) over the full row (the CN CTAs of a cluster own a row)
   const float* ln_gamma;
   const float* ln_beta;
@@ -231,13 +236,110 @@ __device__ __forceinline__ void stage_fragment(const float (&acc)[NACC], int j0,
   }
 }
 
+// Output staging of one consumer warpgroup for epilogue_tma: its four warps' share of kStgBytes, 33 KiB, a multiple of
+// 1024 bytes, so that every box in it starts on a swizzle-pattern boundary. 32 KiB hold the boxes, the last 1 KiB the
+// tile's bias (BN <= 256 floats).
+constexpr int kWgStgBytes = 4 * kStgBytesPerWarp;
+constexpr int kWgBoxBytes = 32 * 1024;
+constexpr int kOutBoxCols = 32;   // columns per TMA store box: every BN is a whole number of boxes
+
+// This warpgroup's 64 rows x BN columns of the tile out through TMA (PE_EPI_F16 / GELU_F16 / F32 / RESID_F32 /
+// TANH_F32, no row remap, n % 8 == 0). The arithmetic per element is epilogue_chunk16's fast path, in the same order:
+// acc + bias, epi_act, + resid, one rounding. Results go straight from the accumulator fragments into 64-row x 32-column
+// boxes in the swizzle of the output tensor map: fp16 rows are 64 bytes (SWIZZLE_64B: 16-byte chunk c of row r sits at
+// c ^ ((r >> 1) & 3)), fp32 rows 128 bytes (SWIZZLE_128B: c ^ (r & 7)), so the 8 rows a warp instruction writes land
+// in distinct banks. TMA clips rows >= m and columns >= n. The staging holds 8 fp16 or 4 fp32 boxes: fp32 tiles wider
+// than 128 columns go out in several passes. PE_EPI_RESID_F32 first loads the residual boxes into the staging with TMA
+// (tm_r, the output's layout) and adds each element in place. The stores are left in flight: the next pass, or the
+// next tile's epilogue, waits for them to have read the staging before it writes there. The bias and the residual
+// come through shared memory rather than registers: the accumulators already hold up to 128 of them.
+template <int EPI, int BN>
+__device__ __forceinline__ void epilogue_tma(const GemmParams& p, const CUtensorMap* tm_c, const CUtensorMap* tm_r,
+                                             const float (&acc)[BN / 2], uint8_t* stg, uint32_t stg_addr,
+                                             uint32_t res_bar, uint32_t& res_phase, int row_wg, int col_tile, int wg,
+                                             int lane, bool issuer) {
+  constexpr bool kHalfOut = (EPI == PE_EPI_F16 || EPI == PE_EPI_GELU_F16);
+  constexpr int kRowBytes = kOutBoxCols * (kHalfOut ? 2 : 4);
+  constexpr int kBoxBytes = 64 * kRowBytes;
+  constexpr int kBoxes = BN / kOutBoxCols;
+  constexpr int kPass = kBoxes < kWgBoxBytes / kBoxBytes ? kBoxes : kWgBoxBytes / kBoxBytes;
+  static_assert(kWgBoxBytes + 256 * 4 <= kWgStgBytes, "boxes + bias exceed a warpgroup's staging");
+  float* bias_s = reinterpret_cast<float*>(stg + kWgBoxBytes);
+  const int t = threadIdx.x & 127;
+  const int r0 = (t >> 5) * 16 + (lane >> 2);   // rows r0 and r0 + 8 of the warpgroup's 64
+  const int cq = (lane & 3) * 2;                // columns cq and cq + 1 of every 8
+#pragma unroll
+  for (int b0 = 0; b0 < kBoxes; b0 += kPass) {
+    if (issuer) {
+      tma_store_wait_read();   // the stores issued from this staging before have read it
+      if (EPI == PE_EPI_RESID_F32) {
+        const int nb = (kBoxes - b0 < kPass ? kBoxes - b0 : kPass);
+        int boxes = 0;
+        if (row_wg < p.m)
+          for (int b = 0; b < nb && col_tile + (b0 + b) * kOutBoxCols < p.n; ++b) boxes = b + 1;
+        mbar_arrive_expect_tx_addr(res_bar, static_cast<uint32_t>(boxes * kBoxBytes));
+        for (int b = 0; b < boxes; ++b)
+          tma_load_2d_addr(stg_addr + static_cast<uint32_t>(b * kBoxBytes), tm_r, res_bar,
+                           col_tile + (b0 + b) * kOutBoxCols, row_wg);
+      }
+    }
+    if (b0 == 0) {   // bias of the tile's columns (0 where there is none: the register path adds 0 too)
+      for (int c = t; c < BN; c += 128) {
+        const int col = col_tile + c;
+        bias_s[c] = p.bias != nullptr && col < p.n ? __ldg(p.bias + col) : 0.f;
+      }
+    }
+    named_barrier_id(3 + wg, 128);
+    if (EPI == PE_EPI_RESID_F32) {
+      mbar_wait_addr(res_bar, res_phase);
+      res_phase ^= 1u;
+    }
+#pragma unroll
+    for (int i = 0; i < kPass * 4; ++i) {
+      const int j = b0 * 4 + i, jj = i & 3;
+      if (j >= BN / 8) break;
+      const float2 bv = *reinterpret_cast<const float2*>(bias_s + 8 * j + cq);
+      uint8_t* box = stg + (i >> 2) * kBoxBytes;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = r0 + 8 * h;
+        const float x0 = acc[4 * j + 2 * h] + bv.x, x1 = acc[4 * j + 2 * h + 1] + bv.y;
+        if (kHalfOut) {
+          *reinterpret_cast<__half2*>(box + r * kRowBytes + ((jj ^ ((r >> 1) & 3)) << 4) + cq * 2) =
+              __floats2half2_rn(epi_act<EPI>(x0), epi_act<EPI>(x1));
+        } else {
+          float2* o = reinterpret_cast<float2*>(box + r * kRowBytes + (((2 * jj + (lane & 3) / 2) ^ (r & 7)) << 4) +
+                                                (lane & 1) * 8);
+          const float2 rv = EPI == PE_EPI_RESID_F32 ? *o : make_float2(0.f, 0.f);
+          *o = make_float2(epi_act<EPI>(x0) + rv.x, epi_act<EPI>(x1) + rv.y);
+        }
+      }
+    }
+    fence_proxy_async_smem();   // the generic-proxy writes above become visible to the TMA engine's reads
+    named_barrier_id(3 + wg, 128);
+    if (issuer) {
+      if (row_wg < p.m) {
+#pragma unroll
+        for (int b = 0; b < kPass; ++b) {
+          const int col = col_tile + (b0 + b) * kOutBoxCols;
+          if (b0 + b < kBoxes && col < p.n) tma_store_2d(tm_c, stg_addr + static_cast<uint32_t>(b * kBoxBytes), col, row_wg);
+        }
+      }
+      tma_store_commit();
+    }
+  }
+}
+
 template <int EPI, int BN>
 __global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b, const GemmParams p) {
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
+                  const __grid_constant__ CUtensorMap tm_c, const __grid_constant__ CUtensorMap tm_r,
+                  const GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[kMaxStages];
   __shared__ __align__(8) uint64_t empty_bar[kMaxStages];
   __shared__ __align__(8) uint64_t ln_bar[2];     // PE_EPI_RESID_LN: "every CTA of the row has published its statistics"
+  __shared__ __align__(8) uint64_t res_bar[2];    // epilogue_tma: a consumer warpgroup's residual boxes have landed
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -262,12 +364,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
   if (warp == kProducerWarp && lane == 0) {
     tma_prefetch_desc(&tm_a);
     tma_prefetch_desc(&tm_b);
+    if (p.tma_out) tma_prefetch_desc(&tm_c);
+    if (p.tma_out && EPI == PE_EPI_RESID_F32) tma_prefetch_desc(&tm_r);
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full_bar[s], 1);
       // one release per consumer warpgroup of every CTA that reads what this CTA writes into the stage
       mbar_init(&empty_bar[s], static_cast<uint32_t>(2 * (p.cm + p.cn - 1)));
     }
     for (int s = 0; s < 2; ++s) mbar_init(&ln_bar[s], static_cast<uint32_t>(p.cn));
+    for (int s = 0; s < 2; ++s) mbar_init(&res_bar[s], 1);
     fence_barrier_init();
   }
   __syncthreads();
@@ -346,6 +451,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
     const uint32_t empty_remote0 =
         csize > 1 ? mapa_shared(empty_addr0, static_cast<uint32_t>(lane < csize ? lane : 0)) : empty_addr0;
     float* stg = reinterpret_cast<float*>(smem_gen + p.stg_offset + warp * kStgBytesPerWarp);
+    const bool store_issuer = (threadIdx.x & 127) == 0;   // issues and waits for this warpgroup's TMA stores
+    const uint32_t res_bar_addr = smem_u32(&res_bar[wg]);
+    uint32_t res_phase = 0u;
     int stage = 0;
     uint32_t phase = 0;
     int par = 0;
@@ -353,13 +461,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
     for (int sup = cluster_id; sup < num_supers; sup += num_clusters) {
       const int m_blk = (sup % p.num_super_m) * p.cm + m_rank;
       const int n_blk = (sup / p.num_super_m) * p.cn + n_rank;
+      // trace slots 2, 3, 5 for a CTA's first tile, 7, 8, 10 for its second
+      const int tslot = trace == nullptr || threadIdx.x != 0 ? -1 : (sup == cluster_id ? 0 : (sup == cluster_id + num_clusters ? 5 : -1));
       float acc[BN / 2];
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
       int prev_stage = -1;
       for (int kb = 0; kb < num_k_blocks; ++kb) {
         mbar_wait_addr(full_addr0 + static_cast<uint32_t>(stage) * 8u, phase);
-        if (trace != nullptr && sup == cluster_id && kb == 0 && threadIdx.x == 0) trace[2] = clock64();
+        if (tslot >= 0 && kb == 0) trace[2 + tslot] = clock64();
         const uint32_t sa = smem_base + static_cast<uint32_t>(stage) * stage_bytes;
         const uint64_t da = wgmma_desc_kmajor_sw128(sa + a_wg_off);
         const uint64_t db = wgmma_desc_kmajor_sw128(sa + kABytes);
@@ -383,7 +493,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
         if (csize > 1) mbar_arrive_remote(e);
         else mbar_arrive_addr(e);
       }
-      if (trace != nullptr && sup == cluster_id && threadIdx.x == 0) trace[3] = clock64();
+      if (tslot >= 0) trace[3 + tslot] = clock64();
       // the staging aliases the ring when each CTA has one tile: the other warpgroup may still be reading it
       if (p.stg_offset == 0) named_barrier<1>(kConsumerThreads);
       const int row0 = m_blk * kBlockM + warp * 16;   // this warp's 16 accumulator rows
@@ -477,6 +587,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
           }
         }
         par ^= 1;
+      } else if (p.tma_out) {
+        const uint32_t wg_stg = static_cast<uint32_t>(p.stg_offset + wg * kWgStgBytes);
+        epilogue_tma<EPI, BN>(p, &tm_c, &tm_r, acc, smem_gen + wg_stg, smem_base + wg_stg, res_bar_addr, res_phase,
+                              m_blk * kBlockM + wg * 64, n_blk * BN, wg, lane, store_issuer);
       } else {
         // ---- registers -> staged 16 x 32 chunk -> (bias, activation, residual, convert) -> coalesced stores
 #pragma unroll
@@ -488,8 +602,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
           __syncwarp();
         }
       }
-      if (trace != nullptr && sup == cluster_id && threadIdx.x == 0) trace[5] = clock64();
+      if (tslot >= 0) trace[5 + tslot] = clock64();
     }
+    // the staging must outlive the stores' reads of it, and their writes must be done when the grid completes
+    if (p.tma_out && store_issuer) tma_store_wait_all();
   }
 
   __syncthreads();
@@ -535,6 +651,39 @@ static int encode_f16_2d(CUtensorMap* map, const void* ptr, uint64_t rows, uint6
     return PE_ERR_CUDA;
   }
   return PE_OK;
+}
+
+// Row-major [rows, cols] fp16 or fp32 output -> boxes of 64 rows x kOutBoxCols columns, the layout epilogue_tma
+// writes: 64-byte fp16 rows in the 64-byte swizzle, 128-byte fp32 rows in the 128-byte swizzle. Stores are clipped at
+// the tensor's edges.
+static int encode_out_2d(CUtensorMap* map, void* ptr, uint64_t rows, uint64_t cols, bool half) {
+  EncodeTiledFn fn = get_encode_fn();
+  if (fn == nullptr) return PE_ERR_CUDA;
+  const uint64_t esize = half ? 2 : 4;
+  const cuuint64_t dims[2] = {cols, rows};
+  const cuuint64_t strides[1] = {cols * esize};
+  const cuuint32_t box[2] = {kOutBoxCols, 64};
+  const cuuint32_t estr[2] = {1, 1};
+  const CUresult rc = fn(map, half ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, ptr, dims,
+                         strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                         half ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (rc != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeTiled failed (CUresult %d) for the [%llu x %llu] GEMM output", static_cast<int>(rc),
+              static_cast<unsigned long long>(rows), static_cast<unsigned long long>(cols));
+    return PE_ERR_CUDA;
+  }
+  return PE_OK;
+}
+
+// PE_GEMM_REG_STORE=1 stores every GEMM output from registers, as the patch embedding always does (A/B timing and the
+// test that both store paths give the same bits). Read once per process.
+static bool gemm_tma_store_enabled() {
+  static const bool on = [] {
+    const char* e = getenv("PE_GEMM_REG_STORE");
+    return !(e != nullptr && e[0] == '1');
+  }();
+  return on;
 }
 
 static long long* g_gemm_trace = nullptr;   // set by pe_debug_gemm_trace
@@ -588,7 +737,8 @@ GemmPlan plan_gemm(int m, int n, int k, int epilogue) {
 }
 
 template <int EPI, int BN>
-static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream) {
+static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc, const CUtensorMap& tr,
+                       const GemmParams& p, cudaStream_t stream) {
   static bool configured = false;
   // the attribute bounds DYNAMIC shared memory; static barriers live outside it (227 KiB total per CTA)
   const int max_smem = kPipeSmemBudget + kStgBytes + kLnAreaBytes + 1024;
@@ -618,27 +768,28 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmP
   attr[1].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = pdl_enabled() ? 2 : 1;
-  PE_CUDA(cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<EPI, BN>, ta, tb, p));
+  PE_CUDA(cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<EPI, BN>, ta, tb, tc, tr, p));
   count_launches(1);
   return PE_OK;
 }
 
 // The wgmma tile width is a compile-time operand: one kernel per BN (a multiple of 32 up to kMaxBN).
 template <int EPI, int kMaxBN = 256>
-static int launch_gemm_bn(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream) {
+static int launch_gemm_bn(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc, const CUtensorMap& tr,
+                          const GemmParams& p, cudaStream_t stream) {
   switch (p.block_n) {
-    case 32: return launch_gemm<EPI, 32>(ta, tb, p, stream);
-    case 64: return launch_gemm<EPI, 64>(ta, tb, p, stream);
-    case 96: return launch_gemm<EPI, 96>(ta, tb, p, stream);
-    case 128: return launch_gemm<EPI, 128>(ta, tb, p, stream);
+    case 32: return launch_gemm<EPI, 32>(ta, tb, tc, tr, p, stream);
+    case 64: return launch_gemm<EPI, 64>(ta, tb, tc, tr, p, stream);
+    case 96: return launch_gemm<EPI, 96>(ta, tb, tc, tr, p, stream);
+    case 128: return launch_gemm<EPI, 128>(ta, tb, tc, tr, p, stream);
     default: break;
   }
   if constexpr (kMaxBN > 128) {
     switch (p.block_n) {
-      case 160: return launch_gemm<EPI, 160>(ta, tb, p, stream);
-      case 192: return launch_gemm<EPI, 192>(ta, tb, p, stream);
-      case 224: return launch_gemm<EPI, 224>(ta, tb, p, stream);
-      case 256: return launch_gemm<EPI, 256>(ta, tb, p, stream);
+      case 160: return launch_gemm<EPI, 160>(ta, tb, tc, tr, p, stream);
+      case 192: return launch_gemm<EPI, 192>(ta, tb, tc, tr, p, stream);
+      case 224: return launch_gemm<EPI, 224>(ta, tb, tc, tr, p, stream);
+      case 256: return launch_gemm<EPI, 256>(ta, tb, tc, tr, p, stream);
       default: break;
     }
   }
@@ -704,12 +855,26 @@ int linear_impl(const void* a, const void* w, const void* bias, const void* resi
   if (rc != PE_OK) return rc;
   rc = encode_f16_2d(&tb, w, static_cast<uint64_t>(n), static_cast<uint64_t>(k), static_cast<uint32_t>(p.block_n / p.cm));
   if (rc != PE_OK) return rc;
+  // TMA stores need 16-byte aligned rows; n % 8 == 0 is also where the register path adds bias and residual on every
+  // element (its per-element tail path skips the + 0 of a missing bias or residual), so both paths give the same bits.
+  CUtensorMap tc = {}, tr = {};   // output; residual (read in the output's layout)
+  const bool half_out = epilogue == PE_EPI_F16 || epilogue == PE_EPI_GELU_F16;
+  p.tma_out = gemm_tma_store_enabled() && rows_per_item == 0 && (n & 7) == 0 &&
+              (reinterpret_cast<uintptr_t>(out) & 15) == 0 && (resid == nullptr || (reinterpret_cast<uintptr_t>(resid) & 15) == 0);
+  if (p.tma_out) {
+    rc = encode_out_2d(&tc, out, static_cast<uint64_t>(m), static_cast<uint64_t>(n), half_out);
+    if (rc != PE_OK) return rc;
+    if (epilogue == PE_EPI_RESID_F32) {
+      rc = encode_out_2d(&tr, const_cast<void*>(resid), static_cast<uint64_t>(m), static_cast<uint64_t>(n), false);
+      if (rc != PE_OK) return rc;
+    }
+  }
   switch (epilogue) {
-    case PE_EPI_F16: return launch_gemm_bn<PE_EPI_F16>(ta, tb, p, stream);
-    case PE_EPI_GELU_F16: return launch_gemm_bn<PE_EPI_GELU_F16>(ta, tb, p, stream);
-    case PE_EPI_RESID_F32: return launch_gemm_bn<PE_EPI_RESID_F32>(ta, tb, p, stream);
-    case PE_EPI_F32: return launch_gemm_bn<PE_EPI_F32>(ta, tb, p, stream);
-    case PE_EPI_TANH_F32: return launch_gemm_bn<PE_EPI_TANH_F32>(ta, tb, p, stream);
+    case PE_EPI_F16: return launch_gemm_bn<PE_EPI_F16>(ta, tb, tc, tr, p, stream);
+    case PE_EPI_GELU_F16: return launch_gemm_bn<PE_EPI_GELU_F16>(ta, tb, tc, tr, p, stream);
+    case PE_EPI_RESID_F32: return launch_gemm_bn<PE_EPI_RESID_F32>(ta, tb, tc, tr, p, stream);
+    case PE_EPI_F32: return launch_gemm_bn<PE_EPI_F32>(ta, tb, tc, tr, p, stream);
+    case PE_EPI_TANH_F32: return launch_gemm_bn<PE_EPI_TANH_F32>(ta, tb, tc, tr, p, stream);
     default: set_error("pe_linear: unknown epilogue %d", epilogue); return PE_ERR_INVALID;
   }
 }
@@ -761,7 +926,8 @@ int linear_ln_impl(const void* a, const void* w, const void* bias, const void* r
   if (rc != PE_OK) return rc;
   rc = encode_f16_2d(&tb, w, static_cast<uint64_t>(n), static_cast<uint64_t>(k), static_cast<uint32_t>(p.block_n));
   if (rc != PE_OK) return rc;
-  return launch_gemm_bn<PE_EPI_RESID_LN, 128>(ta, tb, p, stream);
+  const CUtensorMap tc = {}, tr = {};   // unused: this epilogue stores from registers
+  return launch_gemm_bn<PE_EPI_RESID_LN, 128>(ta, tb, tc, tr, p, stream);
 }
 
 // Host-only: the plan and launch geometry pe_linear would use for this shape (no device needed).
