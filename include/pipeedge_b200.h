@@ -265,6 +265,48 @@ int pe_link_check(pe_link* link);                          /* PE_OK, or the prot
 int pe_link_debug_read(pe_link* link, unsigned long long seq, size_t offset, void* host_dst, size_t bytes);
 #define PE_LINK_HEADER_BYTES 16384   /* slot = [header | payload]; scale f32[512] of tensor t at 256 + 4096 t, shift 2048 later */
 
+/* ---- Host rings: the hops of a data rank without a GPU ------------------------------------------------
+ * A data rank outside the stage pipeline that has no CUDA device (`runtime.py -d cpu`, or no visible GPU) moves its
+ * inputs and results through rings in POSIX shared memory that it creates: R slots of [16 KiB header | payload] and a
+ * monotonic full[s] / free[s] counter pair per slot, both in the segment (4 KiB of counters, then the slots). A
+ * producer publishes a slot's k-th use with a release store full[s] = k + 1 and a ticket {items, dim1} on the hop's
+ * socket; the consumer acquires full[s], checks the header and releases the slot with a release store free[s] = k + 1.
+ * Every wait is bounded by PIPEEDGE_LINK_TIMEOUT_S. The segment is named by the caller (`/name`, at most 62 more
+ * characters) and unlinked as soon as both ends have mapped it or the handshake failed.
+ *
+ * Host-only entry points (pe_hostring_*) never touch the CUDA runtime. The stage at the other end of such a hop opens
+ * it with pe_link_open as usual: the handshake tells it that the peer is a host ring, and it maps the segment and
+ * registers it with CUDA (cudaHostRegisterMapped | Portable). A last stage's send kernel then stores raw f32 results
+ * straight into the mapped slots; a first stage waits for each input with pe_link_shm_wait, feeds it to its host-fed
+ * ring with pe_pipe_submit (a copy-engine transfer out of the registered slot) and hands the slot back with
+ * pe_link_shm_release. */
+typedef struct pe_hostring pe_hostring;
+/* Data rank: create the segment `name` for the hop on `fd` and hand it to the stage. Producer (inputs): the geometry is
+ * `slot_payload_bytes` per slot and `n_slots` in [2,8]. Consumer (results): pass 0, 0; the last stage's hello names it. */
+int pe_hostring_create(int fd, const char* name, int is_producer, size_t slot_payload_bytes, int n_slots,
+                       pe_hostring** out);
+/* The stage's side of pe_hostring_create without a GPU (tests; what pe_link_open does less the CUDA registration). */
+int pe_hostring_attach(int fd, int is_producer, size_t slot_payload_bytes, int n_slots, pe_hostring** out);
+int pe_hostring_close(pe_hostring* ring);   /* unmaps; `fd` stays the caller's */
+size_t pe_hostring_slot_bytes(const pe_hostring* ring);
+/* Producer: wait for a free slot, write a raw header and `bytes` of payload, publish it and send the ticket
+ * {items, dim1}. A payload larger than a slot is refused before anything is written. */
+int pe_hostring_publish(pe_hostring* ring, const void* data, size_t bytes, int items, long long dim1);
+int pe_hostring_close_input(pe_hostring* ring);   /* producer: the closing ticket */
+/* Consumer: the next ticket (blocks; 1 = the producer closed), then its payload - the header must name `items` and
+ * `bytes` (a raw payload, or one raw f32 tensor of items x n values) - valid until pe_hostring_release. */
+int pe_hostring_next(pe_hostring* ring, long long* ticket2);
+int pe_hostring_wait(pe_hostring* ring, int items, size_t bytes, const void** data);
+int pe_hostring_release(pe_hostring* ring);
+/* The stage's end of a host ring (a pe_link from pe_link_open whose peer is a data rank without a GPU). */
+int pe_link_is_shm(const pe_link* link);
+/* First stage: wait on the host for the payload the last ticket (pe_link_ticket_recv) announced; *src = the payload in
+ * registered host memory, a pinned source for pe_pipe_submit. */
+int pe_link_shm_wait(pe_link* link, int items, size_t bytes, const void** src);
+/* ... then hand its slot back behind the copy on `stream` (the pipe's copy stream): a one-thread kernel stores free[s]
+ * with st.release.sys into mapped host memory. */
+int pe_link_shm_release(pe_link* link, void* stream);
+
 /* ---- Per-rank stage loop ---------------------------------------------------------------------------
  * Replaces `TensorWorkThread.run` and the queue hand-offs of `DistP2pPipelineStage` (`p2p/__init__.py:261-295,
  * 373-394,442-450`): a stage's micro-batch (link get -> kernels -> link put) is captured once into a CUDA graph;

@@ -96,6 +96,18 @@ SYMBOLS = {
     'pe_link_ticket_recv': (c_int, [c_void_p, POINTER(c_longlong)]),
     'pe_link_check': (c_int, [c_void_p]),
     'pe_link_debug_read': (c_int, [c_void_p, c_ulonglong, c_size_t, c_void_p, c_size_t]),
+    'pe_hostring_create': (c_int, [c_int, c_char_p, c_int, c_size_t, c_int, POINTER(c_void_p)]),
+    'pe_hostring_attach': (c_int, [c_int, c_int, c_size_t, c_int, POINTER(c_void_p)]),
+    'pe_hostring_close': (c_int, [c_void_p]),
+    'pe_hostring_slot_bytes': (c_size_t, [c_void_p]),
+    'pe_hostring_publish': (c_int, [c_void_p, c_void_p, c_size_t, c_int, c_longlong]),
+    'pe_hostring_close_input': (c_int, [c_void_p]),
+    'pe_hostring_next': (c_int, [c_void_p, POINTER(c_longlong)]),
+    'pe_hostring_wait': (c_int, [c_void_p, c_int, c_size_t, POINTER(c_void_p)]),
+    'pe_hostring_release': (c_int, [c_void_p]),
+    'pe_link_is_shm': (c_int, [c_void_p]),
+    'pe_link_shm_wait': (c_int, [c_void_p, c_int, c_size_t, POINTER(c_void_p)]),
+    'pe_link_shm_release': (c_int, [c_void_p, c_void_p]),
     'pe_pipe_create': (c_int, [c_void_p, c_void_p, c_void_p, POINTER(c_void_p)]),
     'pe_pipe_destroy': (c_int, [c_void_p]),
     'pe_pipe_stream': (c_void_p, [c_void_p]),

@@ -12,7 +12,7 @@ PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG_DIR, 'csrc')
 OBJ_DIR = os.path.join(CSRC, 'build')
 LIB_PATH = os.path.join(PKG_DIR, 'libpipeedge_b200.so')
-SOURCES = ['api.cu', 'gemm_wgmma.cu', 'layernorm.cu', 'attention.cu', 'attention_wgmma.cu', 'quant.cu', 'stage.cu', 'edges.cu', 'hop.cu', 'link.cu', 'pipe.cu']
+SOURCES = ['api.cu', 'gemm_wgmma.cu', 'layernorm.cu', 'attention.cu', 'attention_wgmma.cu', 'quant.cu', 'stage.cu', 'edges.cu', 'hop.cu', 'link.cu', 'hostring.cu', 'pipe.cu']
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
 # -fmad=false is NOT set globally: the quantisation kernels use explicit _rn intrinsics where bit-exactness
 # matters, everything else may contract.

@@ -773,15 +773,26 @@ class DistP2pPipelineStage:
         self._create_stage(rank_src, rank_dst, work_cb, results_cb)
 
     # ------------------------------------------------------------------ native pipeline selection
+    def _host_feeder(self) -> bool:
+        """A data rank outside the stage pipeline (no worker, both ranks set) without a CUDA device: the native pipeline
+        serves it through rings in shared memory (`_native.NativeHostFeeder`); the Python-thread path cannot."""
+        rank_src, rank_dst, work_cb, results_cb = self._args
+        return work_cb is None and results_cb is not None and rank_src is not None and rank_dst is not None and \
+            not torch.cuda.is_available()
+
     def _native_capable(self) -> bool:
         """Whether THIS rank's role can run on the native pipeline (csrc/pipe.cu): a native shard as the worker, hooks
         that the link kernels account for, the reference's ring topology with the data rank on the first stage - or the
-        data rank outside the stage pipeline (no worker, both ranks set), which feeds the first stage through a relay."""
+        data rank outside the stage pipeline (no worker, both ranks set), which feeds the first stage through a relay,
+        or, without a CUDA device, through a ring in shared memory. A rank without a CUDA device is capable only in
+        that role, or idle."""
         rank_src, rank_dst, work_cb, results_cb = self._args
-        if os.environ.get('PIPEEDGE_NATIVE', '1') == '0' or not torch.cuda.is_available():
+        if os.environ.get('PIPEEDGE_NATIVE', '1') == '0':
             return False
         if rank_src is None and rank_dst is None and work_cb is None and results_cb is None:
             return True    # idle rank: neutral
+        if not torch.cuda.is_available() and not self._host_feeder():
+            return False
         try:
             from ._native import shard_is_native   # pylint: disable=import-outside-toplevel
         except ImportError:
@@ -801,11 +812,19 @@ class DistP2pPipelineStage:
     def _choose_native(self) -> bool:
         capable = self._native_capable()
         if dist.is_initialized() and dist.get_world_size() > 1:
-            if os.environ.get('PIPEEDGE_NATIVE', '1') == '0' or not torch.cuda.is_available():
-                return False   # the same on every rank: nobody enters the vote
-            vote = torch.tensor([1 if capable else 0], dtype=torch.int)
+            # Every rank votes, with or without a CUDA device: [capable, -(host feeder), -(has a CUDA device)], MIN.
+            # A data rank without a GPU outside the stage pipeline needs the native pipeline; so does the rest of the
+            # world when any rank has a GPU (a world without one runs the Python threads over Gloo, as before).
+            host_feeder = self._host_feeder()
+            vote = torch.tensor([1 if capable else 0, -1 if host_feeder else 0, -1 if torch.cuda.is_available() else 0],
+                                dtype=torch.int)
             dist.all_reduce(vote, op=dist.ReduceOp.MIN)    # control plane (Gloo); every rank builds a stage object
-            return bool(vote[0])
+            native = bool(vote[0] == 1)
+            if not native and int(vote[1]) < 0 and int(vote[2]) < 0:
+                raise RuntimeError("the data rank has no CUDA device: only the native pipeline can serve it, and not "
+                                   "every rank can run it (PIPEEDGE_NATIVE=0, exchange hooks, or a shard it does not "
+                                   "support); give the data rank a GPU or run every rank natively")
+            return native
         return capable and self._args[0] is None and self._args[1] is None
 
     def _create_stage(self, rank_src, rank_dst, work_cb, results_cb):
@@ -840,6 +859,9 @@ class DistP2pPipelineStage:
             if work_cb is not None:
                 from ._native import NativeStage   # pylint: disable=import-outside-toplevel
                 self._native = NativeStage(rank_src, rank_dst, work_cb, results_cb)
+            elif results_cb is not None and self._host_feeder():   # ... outside the stage pipeline, without a GPU
+                from ._native import NativeHostFeeder   # pylint: disable=import-outside-toplevel
+                self._native = NativeHostFeeder(rank_src, rank_dst, results_cb)
             elif results_cb is not None:   # the data rank outside the stage pipeline
                 from ._native import NativeFeeder   # pylint: disable=import-outside-toplevel
                 self._native = NativeFeeder(rank_src, rank_dst, results_cb)
@@ -934,7 +956,7 @@ class DistP2pPipelineStage:
     @property
     def native(self):
         """The `_native.NativeStage` driving this rank (a `_native.NativeFeeder` on a data rank outside the stage
-        pipeline), or None (Python threads / idle rank)."""
+        pipeline, a `_native.NativeHostFeeder` on one without a CUDA device), or None (Python threads / idle rank)."""
         return self._native
 
     def prepare(self, ubatch: int, dim1: int = 0) -> None:

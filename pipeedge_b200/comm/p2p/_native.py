@@ -10,7 +10,11 @@ per-micro-batch host work runs in C with the GIL released:
 * a data rank outside the stage pipeline (`NativeFeeder`) owns no shard: its graph is one relay kernel that moves each
   input micro-batch, bytes unchanged, from its host-fed ring into the first stage's ring (`pe_pipe_capture_relay`);
   the first stage receives it as a raw payload from a peer link. The first stage tells the feeder its input geometry
-  over their hop's socket before the link opens (`send_input_geometry`).
+  over their hop's socket before the link opens (`send_input_geometry`);
+* such a data rank without a CUDA device (`NativeHostFeeder`) never touches CUDA: its hops are rings in shared memory
+  (`pe_hostring_*`). The last stage's send kernel stores results into one (its `pe_link_open` learns from the
+  handshake that the peer is such a ring); the first stage feeds inputs out of the other into a host-fed ring, as a
+  data rank that owns it does (`NativeStage._shm_loop`).
 
 Activations cross hops as peer-memory stores synchronised by device-polled flags (`csrc/link.cu`); QuantPipe
 quantisation (`-q`, the shard's `quant_bit` buffer) is fused into the send kernel and undone by the receive kernel, so
@@ -273,6 +277,7 @@ class NativeStage:
         self._pipe = ctypes.c_void_p()
         self._links = []                      # every pe_link this rank opened (closed at shutdown)
         self._link_in = self._link_out = self._link_res = None
+        self._shm_in = None                   # first stage fed by a data rank without a GPU: its shared-memory ring
         self._socks = []
         self._inputs = {}                     # (ubatch, dim1) -> persistent input tensors
         self._keep = collections.deque(maxlen=link_slots() + 2)   # sources of in-flight input copies
@@ -336,14 +341,19 @@ class NativeStage:
                 if self._raw_in:   # the feeder owns no shard: it sizes the link from this
                     send_input_geometry(sock, *max_input_geometry(shard))
                 peer_in = self._open_link(sock, False, 0)
-        if self._is_data:
+        # fed by a data rank without a GPU: its inputs wait in a shared-memory ring, and this rank feeds them to a
+        # host-fed ring as a data rank that owns the first stage does (`_shm_loop`)
+        self._shm_in = peer_in if self._raw_in and LIB.pe_link_is_shm(peer_in) else None
+        if self._is_data or self._shm_in is not None:
             # inputs arrive from the host; results come back on the hop from the last stage (or a loop-back link)
             in_bytes = max_input_geometry(shard)[0]
             handle = ctypes.c_void_p()
             check(LIB.pe_link_open_host(in_bytes, link_slots(), ctypes.byref(handle)))
             self._links.append(handle)
             self._link_in = handle
-            if peer_out is None:
+            if not self._is_data:
+                self._link_out = peer_out
+            elif peer_out is None:
                 loop = ctypes.c_void_p()
                 check(LIB.pe_link_open_local(out_bytes, link_slots(), 0, ctypes.byref(loop)))
                 self._links.append(loop)
@@ -365,6 +375,8 @@ class NativeStage:
         if self._is_data:
             self._result_shape = tuple(int(d) for d in shard.native_result_item_shape())
             thr = threading.Thread(target=self._guard, args=(self._results_loop,), daemon=True, name='pe-results')
+        elif self._shm_in is not None:
+            thr = threading.Thread(target=self._guard, args=(self._shm_loop,), daemon=True, name='pe-shm-feed')
         else:
             thr = threading.Thread(target=self._guard, args=(self._run_loop,), daemon=True, name='pe-stage')
         if self._record_cbs or self._send_hooks:
@@ -615,6 +627,28 @@ class NativeStage:
                 continue
             check(rc)
 
+    def _shm_loop(self) -> None:
+        """First stage fed by a data rank without a GPU: per ticket, wait for the input in the shared-memory ring, copy
+        it into the host-fed ring and launch the graph (`pe_pipe_submit`, the registered slot as a pinned source), then
+        hand the slot back behind that copy on the copy stream. The data rank's close travels on downstream."""
+        ticket = (ctypes.c_longlong * 2)()
+        src = ctypes.c_void_p()
+        copy_stream = LIB.pe_pipe_copy_stream(self._pipe)
+        while True:
+            rc = LIB.pe_link_ticket_recv(self._shm_in, ticket)
+            if rc == 1 or (rc == 0 and ticket[0] < 0):
+                check(LIB.pe_pipe_close_input(self._pipe))
+                return
+            check(rc)
+            ubatch, dim1 = int(ticket[0]), int(ticket[1])
+            if not LIB.pe_pipe_has_graph(self._pipe, ubatch, dim1):
+                self._capture(ubatch, dim1)
+            x = self._inputs[(ubatch, dim1)][0]   # the graph's input buffer: the size of this shape's inputs
+            nbytes = x.numel() * x.element_size()
+            check(LIB.pe_link_shm_wait(self._shm_in, ubatch, nbytes, ctypes.byref(src)))
+            check(LIB.pe_pipe_submit(self._pipe, src, nbytes, 1, ubatch, dim1))
+            check(LIB.pe_link_shm_release(self._shm_in, copy_stream))
+
     # ------------------------------------------------------------------ common
     def check(self) -> None:
         """Re-raise what killed a native thread."""
@@ -757,3 +791,136 @@ class NativeFeeder(NativeStage):
             self.graph_kernels[(ubatch, dim1)] = kernels.value
             self.variant_kernels[(ubatch, dim1, 0)] = kernels.value
             self.captures += 1
+
+
+def shm_name(src: int, dst: int) -> str:
+    """Name of the shared-memory ring of the hop `src` -> `dst` of a data rank without a GPU (ranks share a node;
+    MASTER_PORT keeps concurrent jobs apart, as `DistP2pContext.sock_path` does)."""
+    return f"/pipeedge_b200_{os.environ.get('MASTER_PORT', '0')}_{src}_{dst}"
+
+
+class NativeHostFeeder:
+    """A data rank outside the stage pipeline WITHOUT a CUDA device (`runtime.py -d cpu`, or no visible GPU) on the
+    native pipeline. It never touches CUDA. Both of its hops are rings in shared memory that it creates
+    (`pe_hostring_create`): `enqueue` converts each micro-batch on the CPU to the first stage's input dtype and publishes
+    it into the input ring, which the first stage copies out of with its copy engine; the last stage's send kernel
+    stores the results into the other ring, and a results thread hands them to `results_cb` in order, as [items, n]
+    fp32 CPU tensors. `rank_dst`: the first stage; `rank_src`: the last stage."""
+
+    def __init__(self, rank_src: int, rank_dst: int, results_cb: Callable):
+        self._rank_src, self._rank_dst = rank_src, rank_dst
+        self._results_cb = results_cb
+        self._ring_in = self._ring_res = None
+        self._socks = []
+        self._geometry = None       # (largest input micro-batch in bytes, dtype, tensor rank) from the first stage
+        self._send_hooks = []       # (hook, args): hook(mbits, seconds, *args) per micro-batch published
+        self._thread = None
+        self._closed = False
+        self.exception: Optional[BaseException] = None
+
+    def init(self, connect_to: Callable, accept_from: Callable) -> None:
+        """Open the hop to the first stage (reading its input geometry first) and the hop from the last one, in
+        ascending order of the sender's rank like every stage; start the results thread."""
+        rank = dist.get_rank() if dist.is_initialized() else 0
+        for _, kind in sorted([(rank, 'send'), (self._rank_src, 'recv')]):
+            handle = ctypes.c_void_p()
+            if kind == 'send':
+                sock = connect_to(self._rank_dst)
+                self._socks.append(sock)
+                self._geometry = recv_input_geometry(sock)
+                check(LIB.pe_hostring_create(sock.fileno(), shm_name(rank, self._rank_dst).encode(), 1,
+                                             self._geometry[0], link_slots(), ctypes.byref(handle)))
+                self._ring_in = handle
+            else:
+                sock = accept_from(self._rank_src)
+                self._socks.append(sock)
+                check(LIB.pe_hostring_create(sock.fileno(), shm_name(self._rank_src, rank).encode(), 0, 0, 0,
+                                             ctypes.byref(handle)))
+                self._ring_res = handle
+        self._thread = threading.Thread(target=self._guard, daemon=True, name='pe-host-results')
+        self._thread.start()
+
+    @property
+    def input_geometry(self) -> Optional[Tuple[int, torch.dtype, int]]:
+        """(largest input micro-batch in bytes, dtype, tensor rank) the first stage announced (after `init()`)."""
+        return self._geometry
+
+    def add_send_timing_hook(self, hook: Callable[..., None], args: tuple) -> None:
+        """`hook(mbits, seconds, *args)` once per micro-batch: the payload in Mbit and the host-clock time its publication
+        took (waiting for a free slot included, as a device send includes waiting for the receiver)."""
+        self._send_hooks.append((hook, args))
+
+    def prepare(self, ubatch: int, dim1: int = 0) -> None:
+        """No-op: this rank captures no graph."""
+
+    def enqueue(self, tensor: torch.Tensor) -> None:
+        """Insert one micro-batch (converted to the first stage's input dtype); blocks while the input ring is full."""
+        self.check()
+        max_bytes, dtype, ndim = self._geometry
+        if tensor.dim() != ndim:
+            raise ValueError(f"native pipeline: a {tensor.dim()}-D input where the first stage takes {ndim}-D ones")
+        ubatch = int(tensor.shape[0])
+        dim1 = int(tensor.shape[1]) if ndim == 2 else 0      # BERT: the sequence length is the payload's
+        if ubatch > max_ubatch():
+            raise ValueError(f"micro-batch of {ubatch} items exceeds PIPEEDGE_MAX_UBATCH={max_ubatch()}")
+        tensor = tensor.detach().to(dtype).contiguous()
+        nbytes = tensor.numel() * tensor.element_size()
+        if nbytes > max_bytes:
+            raise ValueError(f"native pipeline: an input of {nbytes} bytes exceeds the first stage's largest "
+                             f"({max_bytes} bytes)")
+        t0 = time.perf_counter()
+        check(LIB.pe_hostring_publish(self._ring_in, tensor.data_ptr(), nbytes, ubatch, dim1))
+        seconds = time.perf_counter() - t0
+        for hook, args in self._send_hooks:
+            hook(nbytes * 8e-6, seconds, *args)
+
+    def _guard(self) -> None:
+        try:
+            self._results_loop()
+        except BaseException as exc:   # pylint: disable=broad-except
+            self.exception = exc       # re-raised on the owner by check()
+            logger.exception("native pipeline results thread failed")
+
+    def _results_loop(self) -> None:
+        ticket = (ctypes.c_longlong * 2)()
+        data = ctypes.c_void_p()
+        while True:
+            rc = LIB.pe_hostring_next(self._ring_res, ticket)
+            if rc == 1:
+                return
+            check(rc)
+            items, n = int(ticket[0]), int(ticket[1])
+            check(LIB.pe_hostring_wait(self._ring_res, items, items * n * 4, ctypes.byref(data)))
+            buf = (ctypes.c_float * (items * n)).from_address(data.value)
+            out = torch.frombuffer(buf, dtype=torch.float32, count=items * n).clone().view(items, n)
+            check(LIB.pe_hostring_release(self._ring_res))
+            self._results_cb(out)
+
+    def check(self) -> None:
+        """Re-raise what killed the results thread."""
+        if self.exception is not None:
+            raise RuntimeError("the native pipeline's results thread failed") from self.exception
+
+    def shutdown(self, timeout: float = 120.0) -> None:
+        """Close the input (the closing ticket travels down the pipeline and back), wait for the results thread, then -
+        after ALL ranks have drained (barrier) - unmap the rings."""
+        if self._closed:
+            return
+        self._closed = True
+        failure = self.exception
+        if self._ring_in:
+            LIB.pe_hostring_close_input(self._ring_in)
+        if self._thread is not None:
+            self._thread.join(timeout)
+        if dist.is_initialized() and dist.get_world_size() > 1 and failure is None and self.exception is None:
+            drain_barrier()   # no rank unmaps a ring while a neighbour may still use it
+        for handle in (self._ring_in, self._ring_res):
+            if handle:
+                LIB.pe_hostring_close(handle)
+        self._ring_in = self._ring_res = None
+        for sock in self._socks:
+            try:
+                sock.close()
+            except OSError:
+                pass
+        self._socks.clear()

@@ -630,14 +630,15 @@ __global__ void __launch_bounds__(kPutThreads) link_relay_kernel(const RelayArgs
   }
 }
 
-// ------------------------------------------------------------------------------------------------ host helpers
-static unsigned long long default_timeout_ns() {
-  const char* e = getenv("PIPEEDGE_LINK_TIMEOUT_S");
-  double s = e != nullptr ? atof(e) : 30.0;
-  if (s < 0.01) s = 0.01;
-  return static_cast<unsigned long long>(s * 1e9);
+// ------------------------------------------------------------------------------------------------ shared-memory input
+// A first stage fed by a data rank without a GPU copies each input out of the shared-memory ring on its copy stream
+// (pe_pipe_submit); this kernel, enqueued behind that copy, hands the slot back: the copy engine has finished reading it
+// when the kernel starts.
+__global__ void __launch_bounds__(1) link_shm_release_kernel(uint64_t* free_flag, uint64_t value) {
+  st_release_sys(free_flag, value);
 }
 
+// ------------------------------------------------------------------------------------------------ host helpers
 static int sm_count() {
   static int cached = 0;
   if (cached == 0) {
@@ -669,7 +670,7 @@ static int alloc_common(pe_link* l) {
   l->tx.bar_gen = reinterpret_cast<unsigned*>(c + 192);
   l->tx.partials = reinterpret_cast<double*>(c + 256);
   l->rx.status = l->tx.status = status_dev;
-  l->timeout_ns = default_timeout_ns();
+  l->timeout_ns = link_timeout_ns();
   preload_kernels();
   const char* w = getenv("PIPEEDGE_WIRE_F16");
   l->wire_f16 = (w != nullptr && w[0] == '1') ? 1 : 0;
@@ -686,6 +687,7 @@ static void preload_kernels() {
   cudaFuncGetAttributes(&attr, link_put_copy_kernel);
   cudaFuncGetAttributes(&attr, link_put_staged_kernel);
   cudaFuncGetAttributes(&attr, link_relay_kernel);
+  cudaFuncGetAttributes(&attr, link_shm_release_kernel);
   cudaFuncGetAttributes(&attr, link_put_quant_kernel<2>);
   cudaFuncGetAttributes(&attr, link_put_quant_kernel<4>);
   cudaFuncGetAttributes(&attr, link_put_quant_kernel<8>);
@@ -697,20 +699,6 @@ static void preload_kernels() {
   cudaGetLastError();
   done = true;
 }
-
-struct HelloMsg {
-  uint32_t magic;
-  uint32_t n_slots;
-  uint32_t quant_hint;         // the bit-width the producer expects to send (sizes the consumer's receive grid)
-  uint32_t pad;
-  uint64_t slot_bytes;
-  cudaIpcMemHandle_t handle;   // the producer's block (free flags)
-};
-struct ReplyMsg {
-  uint32_t magic;
-  uint32_t status;             // 0 ok
-  cudaIpcMemHandle_t handle;   // the consumer's block (full flags + ring)
-};
 
 int link_check(pe_link* l) {
   if (l == nullptr || l->status_host == nullptr) return PE_OK;
@@ -1038,11 +1026,29 @@ static void free_link(pe_link* l) {
   if (l->quant_work != nullptr) cudaFree(l->quant_work);
   if (l->status_host != nullptr) cudaFreeHost(l->status_host);
   if (l->host_flags != nullptr) cudaFreeHost(l->host_flags);
+  if (l->shm_registered) cudaHostUnregister(l->shm.base);
+  hostring_unmap(&l->shm);
   if (l->kind == 1) {
     if (l->fd >= 0) close(l->fd);
     if (l->fd_peer >= 0) close(l->fd_peer);
   }
   delete l;
+}
+
+// A stage's end of a hop to or from a data rank without a GPU: map the segment named in `handle` and register it with
+// CUDA, so that kernels reach its flags and slots and copy engines read it as pinned memory. *dev = the device alias of
+// the mapping.
+static int map_shm_end(pe_link* l, cudaIpcMemHandle_t handle, int n_slots, size_t slot_bytes, uint8_t** dev) {
+  handle.reserved[sizeof(handle.reserved) - 1] = 0;
+  int rc = hostring_map(handle.reserved, false, n_slots, slot_bytes, &l->shm);
+  if (rc != PE_OK) return rc;
+  PE_CUDA(cudaHostRegister(l->shm.base, l->shm.map_bytes, cudaHostRegisterMapped | cudaHostRegisterPortable));
+  l->shm_registered = true;
+  PE_CUDA(cudaHostGetDevicePointer(reinterpret_cast<void**>(dev), l->shm.base, 0));
+  l->kind = 3;
+  l->n_slots = n_slots;
+  l->slot_bytes = slot_bytes;
+  return PE_OK;
 }
 
 }  // namespace pe
@@ -1090,10 +1096,33 @@ int pe_link_open(int fd, int is_producer, size_t slot_payload_bytes, int n_slots
     }
     ReplyMsg reply = {};
     if (write_all(fd, &hello, sizeof(hello)) != 0 || read_all(fd, &reply, sizeof(reply)) != 0 ||
-        reply.magic != kLinkMagic || reply.status != 0) {
+        (reply.magic != kLinkMagic && reply.magic != kShmMagic) || reply.status != 0) {
       set_error("pe_link_open: handshake with the consumer failed");
       free_link(l);
       return PE_ERR_CUDA;
+    }
+    if (reply.magic == kShmMagic) {
+      // the consumer is a data rank without a GPU: the send kernels store straight into its shared-memory ring, raw
+      // f32 (the host reads the results as they are), and poll its free flags in mapped host memory
+      uint8_t* dev = nullptr;
+      rc = map_shm_end(l, reply.handle, n_slots, l->slot_bytes, &dev);
+      const ReplyMsg ack = {kShmMagic, rc == PE_OK ? 0u : 1u, {}};
+      if (write_all(fd, &ack, sizeof(ack)) != 0 && rc == PE_OK) {
+        set_error("pe_link_open: socket write failed");
+        rc = PE_ERR_CUDA;
+      }
+      if (rc == PE_OK) {
+        l->tx.ring = dev + kShmCtlBytes;
+        l->tx.full = reinterpret_cast<uint64_t*>(dev);
+        l->tx.free_ = reinterpret_cast<const uint64_t*>(dev + kShmFreeOff);
+        l->tx.slot_bytes = l->slot_bytes;
+        l->tx.n_slots = n_slots;
+        l->wire_f16 = 0;
+        rc = alloc_staging(l);
+      }
+      if (rc != PE_OK) { free_link(l); return rc; }
+      *out = l;
+      return PE_OK;
     }
     e = cudaIpcOpenMemHandle(&l->peer_block, reply.handle, cudaIpcMemLazyEnablePeerAccess);
     if (e != cudaSuccess) {
@@ -1113,11 +1142,27 @@ int pe_link_open(int fd, int is_producer, size_t slot_payload_bytes, int n_slots
     HelloMsg hello = {};
     ReplyMsg reply = {};
     reply.magic = kLinkMagic;
-    if (read_all(fd, &hello, sizeof(hello)) != 0 || hello.magic != kLinkMagic || hello.n_slots < 2 ||
-        hello.n_slots > static_cast<uint32_t>(kLinkMaxSlots)) {
+    if (read_all(fd, &hello, sizeof(hello)) != 0 || (hello.magic != kLinkMagic && hello.magic != kShmMagic) ||
+        hello.n_slots < 2 || hello.n_slots > static_cast<uint32_t>(kLinkMaxSlots)) {
       set_error("pe_link_open: handshake with the producer failed");
       free_link(l);
       return PE_ERR_CUDA;
+    }
+    if (hello.magic == kShmMagic) {
+      // the producer is a data rank without a GPU: its inputs are read out of the shared-memory ring by the host
+      // (pe_link_shm_wait) and the copy engine (pe_pipe_submit), and handed back by pe_link_shm_release
+      uint8_t* dev = nullptr;
+      rc = map_shm_end(l, hello.handle, static_cast<int>(hello.n_slots), hello.slot_bytes, &dev);
+      reply.magic = kShmMagic;
+      reply.status = rc == PE_OK ? 0u : 1u;
+      if (write_all(fd, &reply, sizeof(reply)) != 0 && rc == PE_OK) {
+        set_error("pe_link_open: socket write failed");
+        rc = PE_ERR_CUDA;
+      }
+      if (rc != PE_OK) { free_link(l); return rc; }
+      l->shm_free_dev = reinterpret_cast<uint64_t*>(dev + kShmFreeOff);
+      *out = l;
+      return PE_OK;
     }
     l->n_slots = static_cast<int>(hello.n_slots);
     l->quant_hint = static_cast<int>(hello.quant_hint);
@@ -1285,6 +1330,30 @@ int pe_link_ticket_recv(pe_link* link, long long* out2) {
 }
 
 int pe_link_check(pe_link* link) { return pe::link_check(link); }
+
+int pe_link_is_shm(const pe_link* link) { return link != nullptr && link->kind == 3 ? 1 : 0; }
+
+// Consumer end of a shared-memory ring (a first stage fed by a data rank without a GPU): wait on the host (bounded) for
+// the payload the last ticket announced, check its header, *src = the payload in registered host memory.
+int pe_link_shm_wait(pe_link* link, int items, size_t bytes, const void** src) {
+  PE_REQUIRE(link != nullptr && link->kind == 3 && link->is_rx && src != nullptr,
+             "pe_link_shm_wait: not the consumer end of a shared-memory ring");
+  return pe::hostring_read(&link->shm, items, bytes, src);
+}
+
+// ... and hand that slot back to the data rank behind everything enqueued on `stream` so far (the copy out of it): a
+// one-thread kernel raises free[s] with st.release.sys in mapped host memory. No host synchronisation.
+int pe_link_shm_release(pe_link* link, void* stream) {
+  using namespace pe;
+  PE_REQUIRE(link != nullptr && link->kind == 3 && link->is_rx, "pe_link_shm_release: not the consumer end of a shared-memory ring");
+  HostRing& g = link->shm;
+  const uint64_t n = static_cast<uint64_t>(g.n_slots);
+  link_shm_release_kernel<<<1, 1, 0, static_cast<cudaStream_t>(stream)>>>(link->shm_free_dev + g.seq % n, g.seq / n + 1);
+  PE_CUDA(cudaGetLastError());
+  count_launches(1);
+  ++g.seq;
+  return PE_OK;
+}
 
 // Tests: copy `bytes` at `offset` of the slot that holds payload number `seq` to host memory (consumer end; synchronises).
 int pe_link_debug_read(pe_link* link, unsigned long long seq, size_t offset, void* host_dst, size_t bytes) {

@@ -76,13 +76,61 @@ struct PutTensor {
   size_t n;                // elements per item
 };
 
+// The open handshake on a hop's socket. The producer writes a HelloMsg, the consumer answers with a ReplyMsg. A hop to or
+// from a data rank without a GPU carries kShmMagic instead: the data rank has created the ring in POSIX shared memory and
+// names it in `handle` (a NUL-terminated shm_open name). Data rank -> first stage: its HelloMsg carries the name, the
+// stage maps the segment and replies. Last stage -> data rank: the data rank answers the stage's HelloMsg with the name,
+// the stage maps the segment and acknowledges with a ReplyMsg of its own. magic 0 / status != 0: the sender failed.
+constexpr uint32_t kShmMagic = 0x4853454bu;        // "KESH"
+struct HelloMsg {
+  uint32_t magic;
+  uint32_t n_slots;
+  uint32_t quant_hint;         // the bit-width the producer expects to send (sizes the consumer's receive grid)
+  uint32_t pad;
+  uint64_t slot_bytes;
+  cudaIpcMemHandle_t handle;   // the producer's block (free flags), or the shared-memory segment's name
+};
+struct ReplyMsg {
+  uint32_t magic;
+  uint32_t status;             // 0 ok
+  cudaIpcMemHandle_t handle;   // the consumer's block (full flags + ring), or the shared-memory segment's name
+};
+
+// A ring in POSIX shared memory between a data rank without a GPU and a stage (hostring.cu): the slot layout and the
+// monotonic full / free counters of a peer link, both counters in the segment. The host end reads and writes it
+// directly with acquire / release atomics; the stage's end registers it with CUDA (mapped, portable), so that link_put
+// stores results into it and a copy engine reads inputs out of it.
+constexpr size_t kShmCtlBytes = 4096;              // segment = [full u64[R] @0, free u64[R] @kShmFreeOff | R slots]
+constexpr size_t kShmFreeOff = 2048;
+struct HostRing {
+  uint8_t* base = nullptr;     // host mapping
+  size_t map_bytes = 0;
+  size_t slot_bytes = 0;       // header included, a multiple of 4096
+  int n_slots = 0;
+  uint64_t seq = 0;            // payloads published (producer) / released (consumer) so far
+  unsigned long long timeout_ns = 0;
+  uint64_t* full() const { return reinterpret_cast<uint64_t*>(base); }
+  uint64_t* free_() const { return reinterpret_cast<uint64_t*>(base + kShmFreeOff); }
+  uint8_t* slot(uint64_t s) const { return base + kShmCtlBytes + (s % static_cast<uint64_t>(n_slots)) * slot_bytes; }
+};
+
+unsigned long long link_timeout_ns();   // PIPEEDGE_LINK_TIMEOUT_S (default 30 s)
+// Map the segment `name` of R slots of `slot_bytes` (create: a new one, zeroed; else an existing one of that size).
+int hostring_map(const char* name, bool create, int n_slots, size_t slot_bytes, HostRing* r);
+void hostring_unmap(HostRing* r);
+// Consumer: wait (bounded) for the next payload's full flag, check its header against `items` and `bytes`, *data = the
+// payload. The slot stays owned until it is released.
+int hostring_read(HostRing* r, int items, size_t bytes, const void** data);
+// Read exactly n bytes within the link timeout: 0 ok, else an error is set.
+int read_within(int fd, void* buf, size_t n, unsigned long long timeout_ns, const char* what);
+
 }  // namespace pe
 
 // Host-side handle. One object per END of a link; a loop-back link (both ends in one process) is one object.
 struct pe_link {
   int fd = -1;               // ticket channel (Unix-domain stream socket); -1 for a host-fed link
   int fd_peer = -1;          // loop-back only: the other end of the socketpair
-  int kind = 0;              // 0 = peer (cudaIpc), 1 = loop-back, 2 = host-fed
+  int kind = 0;              // 0 = peer (cudaIpc), 1 = loop-back, 2 = host-fed, 3 = shared memory with a host data rank
   bool is_tx = false, is_rx = false;
   size_t slot_bytes = 0;
   int n_slots = 0;
@@ -101,6 +149,9 @@ struct pe_link {
   unsigned long long timeout_ns = 0;
   int wire_f16 = 0;
   int quant_hint = 0;              // bit-width the producer announced at open (0 = raw payloads)
+  pe::HostRing shm;                // kind 3: the segment's host mapping (registered with CUDA)
+  bool shm_registered = false;
+  uint64_t* shm_free_dev = nullptr;   // kind 3 consumer: device alias of the segment's free flags
 };
 
 namespace pe {

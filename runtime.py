@@ -541,6 +541,7 @@ def run_pipeline_p2p(world_size: int, rank: int, model_name: str, model_file: Op
             stage = stage_ranks.index(rank)
         except ValueError:
             stage = None
+        check_host_only_role(stage)
         if stage is None:
             model = None
         else:
@@ -578,7 +579,9 @@ def run_pipeline_p2p(world_size: int, rank: int, model_name: str, model_file: Op
             if model is not None:
                 logger.info("Pipeline stage: %s", 'native' if stage_ctx.native is not None else 'Python threads')
             elif rank == data_rank:   # outside the stage pipeline: it feeds the first stage and collects results
-                logger.info("Data rank: %s", 'native' if stage_ctx.native is not None else 'Python threads')
+                kind = 'Python threads' if stage_ctx.native is None else \
+                    'native (host)' if not torch.cuda.is_available() else 'native'
+                logger.info("Data rank: %s", kind)
             if os.getenv(ENV_ADAPTIVE_QUANT) or monitoring_enabled():
                 stage_ctx.register_send_timing_hook(hop_timing_hook_monitor, (MONITORING_KEY_SEND,))
             if rank == data_rank:
@@ -603,16 +606,29 @@ def run_pipeline_p2p(world_size: int, rank: int, model_name: str, model_file: Op
     return throughput
 
 
+def check_host_only_role(stage: Optional[int]) -> None:
+    """A rank without a CUDA device (`-d cpu`, or no visible GPU) may load data outside the stage pipeline or stay idle,
+    as in the reference; a stage needs the GPU."""
+    if stage is not None and not torch.cuda.is_available():
+        raise RuntimeError(f"runtime.py: no CUDA device for stage {stage} - this build has no CPU fallback")
+
+
 def init_env(device: Optional[str], net_addr: str, net_port: int, net_ifname: str) -> None:
-    """Initialize the PyTorch environment (`runtime.py:581-602`). The compute device is always CUDA here."""
-    if not torch.cuda.is_available():
-        raise RuntimeError("runtime.py: no CUDA device - this build has no CPU fallback")
-    if device is None or device == 'cuda':
-        device = f"cuda:{int(os.environ.get('LOCAL_RANK', '0')) % torch.cuda.device_count()}"
-    devices.DEVICE = torch.device(device)
-    if devices.DEVICE.type != 'cuda':
-        raise RuntimeError(f"runtime.py: device {device} is not a CUDA device")
-    torch.cuda.set_device(devices.DEVICE)
+    """Initialize the PyTorch environment (`runtime.py:581-602`). The compute device is CUDA, except on a rank with
+    `-d cpu` or without a visible GPU: that rank is host-only (`devices.DEVICE` is the CPU) and never creates a CUDA
+    context; with `-d cpu` every GPU is hidden from the process, so that no library can create one either."""
+    if device is not None and torch.device(device).type == 'cpu':
+        os.environ['CUDA_VISIBLE_DEVICES'] = ''
+        devices.DEVICE = torch.device('cpu')
+    elif not torch.cuda.is_available():
+        devices.DEVICE = torch.device('cpu')
+    else:
+        if device is None or device == 'cuda':
+            device = f"cuda:{int(os.environ.get('LOCAL_RANK', '0')) % torch.cuda.device_count()}"
+        devices.DEVICE = torch.device(device)
+        if devices.DEVICE.type != 'cuda':
+            raise RuntimeError(f"runtime.py: device {device} is neither a CUDA device nor the CPU")
+        torch.cuda.set_device(devices.DEVICE)
     os.environ['MASTER_ADDR'] = net_addr
     os.environ['MASTER_PORT'] = str(net_port)
     if net_ifname:
@@ -626,7 +642,8 @@ def main() -> None:
     parser.add_argument("rank", type=int, help="the rank for the current node")
     parser.add_argument("worldsize", type=int, help="the world size (the number of nodes)")
     parser.add_argument("-d", "--device", type=str, default=None,
-                        help="compute device, e.g.: 'cuda', 'cuda:1' (default: cuda:LOCAL_RANK or cuda:rank)")
+                        help="compute device, e.g.: 'cuda', 'cuda:1' (default: cuda:LOCAL_RANK or cuda:rank); 'cpu' only for a "
+                             "data rank outside the stage pipeline or an idle rank")
     parser.add_argument("-s", "--socket-ifname", type=str, default="lo", help="socket interface name")
     parser.add_argument("--addr", type=str, default="127.0.0.1", help="ip address for the master node")
     parser.add_argument("--port", type=int, default=29500, help="communication port for the master node")

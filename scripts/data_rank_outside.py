@@ -1,7 +1,9 @@
 """The data rank inside vs outside the stage pipeline (`runtime.py -D 0` with and without `-r 1,2`).
 
 ViT-Base cut into two stages `[1,24],[25,48]`, unquantised. Inside: ranks 0 (the data rank, stage 0) and 1. Outside:
-rank 0 feeds stage 0 on rank 1 through the relay kernel and collects results from stage 1 on rank 2. Every
+rank 0 feeds stage 0 on rank 1 through the relay kernel and collects results from stage 1 on rank 2. Outside with a
+host data rank: the same ranks, rank 0 without a GPU (CUDA_VISIBLE_DEVICES=''), feeding and collecting through rings in
+shared memory (`NativeHostFeeder`). Every
 configuration runs as its own set of processes; the configurations are interleaved and repeated. Per run it prints:
   * stage0_ms: device time per micro-batch on stage 0 over the timed phase (its first graph launch to the end of its
     last, `NativeStage.timing()`); null on the Python-thread path, which has no such timer;
@@ -39,8 +41,12 @@ def _card() -> dict:
 
 def _worker(rank, port, cfg, args, out_q):
     sys.path.insert(0, ROOT)
+    host = cfg.get('host', False) and rank == 0
+    if host:
+        os.environ['CUDA_VISIBLE_DEVICES'] = ''   # the data rank without a GPU, as `runtime.py -d cpu` makes it
     os.environ.update(MASTER_ADDR='127.0.0.1', MASTER_PORT=str(port), PIPEEDGE_NATIVE='1' if cfg['native'] else '0')
-    torch.cuda.set_device(rank if cfg['own_gpu'] else 0)
+    if not host:
+        torch.cuda.set_device(rank if cfg['own_gpu'] else 0)
     import model_cfg
     import runtime as rt
     from pipeedge_b200.comm.p2p import DistP2pContext
@@ -75,7 +81,8 @@ def _worker(rank, port, cfg, args, out_q):
             count[0] += 1
             cond.notify_all()
 
-    x = synth_input(spec, args.ubatch, seed=1).pin_memory()
+    x = synth_input(spec, args.ubatch, seed=1)
+    x = x if host else x.pin_memory()
     report = {}
     with DistP2pContext(('gloo',), {'world_size': world, 'rank': rank}, on_cmd) as ctx:
         with model_cfg.dist_p2p_pipeline_stage_factory(stage_ranks, 0, rank, s, shard, results_cb) as stage:
@@ -159,7 +166,8 @@ def main() -> None:
     if not torch.cuda.is_available():
         raise SystemExit("data_rank_outside.py measures on a GPU; none is visible")
     configs = [dict(name='inside, one GPU', outside=False, own_gpu=False, native=True),
-               dict(name='outside, one GPU', outside=True, own_gpu=False, native=True)]
+               dict(name='outside, one GPU', outside=True, own_gpu=False, native=True),
+               dict(name='outside, host data rank, one GPU', outside=True, own_gpu=False, native=True, host=True)]
     if torch.cuda.device_count() >= 3:
         configs += [dict(name='outside, GPU per rank', outside=True, own_gpu=True, native=True),
                     dict(name='outside, GPU per rank, PIPEEDGE_NATIVE=0', outside=True, own_gpu=True, native=False)]
