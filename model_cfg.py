@@ -5,7 +5,7 @@ entries point at the native shard classes, and `get_model_config` builds the Hug
 architecture table in `pipeedge_b200.synth` instead of `AutoConfig.from_pretrained` (no network).
 """
 import logging
-from typing import Any, Callable, List, Optional
+from typing import Any, Callable, List, Optional, Tuple, Union
 import torch
 from pipeedge_b200.comm import p2p
 from pipeedge_b200.models import ModuleShard, ModuleShardConfig
@@ -88,10 +88,38 @@ def module_shard_factory(model_name: str, model_file: Optional[str], layer_start
     return shard
 
 
-def dist_p2p_pipeline_stage_factory(stage_ranks: List[int], data_rank: int, rank: int, stage: Optional[int],
-                                    module: Optional[ModuleShard], handle_results_cb: Callable[[Any], None]) \
-        -> p2p.DistP2pPipelineStage:
-    """Get a P2P pipeline stage instance with the reference's rank topology (`model_cfg.py:128-166`)."""
+def replica_neighbours(replica_ranks: List[List[int]], data_rank: int, rank: int) \
+        -> Tuple[Optional[int], Optional[int], Optional[int], Optional[int]]:
+    """(replica, stage, rank_src, rank_dst) of `rank` among R replicas of one stage pipeline (`replica_ranks[k][s]`:
+    replica k's stage s) fed by `data_rank` outside them: its neighbours are those of its own replica, and the data rank
+    is the source of every replica's first stage and the destination of every last one. All None for the data rank and
+    for an idle rank."""
+    for replica, ranks in enumerate(replica_ranks):
+        if rank in ranks:
+            stage = ranks.index(rank)
+            rank_src = data_rank if stage == 0 else ranks[stage - 1]
+            rank_dst = data_rank if stage == len(ranks) - 1 else ranks[stage + 1]
+            return replica, stage, rank_src, rank_dst
+    return None, None, None, None
+
+
+def dist_p2p_pipeline_stage_factory(stage_ranks: Union[List[int], List[List[int]]], data_rank: int, rank: int,
+                                    stage: Optional[int], module: Optional[ModuleShard],
+                                    handle_results_cb: Callable[[Any], None]) -> p2p.DistP2pPipelineStage:
+    """Get a P2P pipeline stage instance with the reference's rank topology (`model_cfg.py:128-166`). `stage_ranks` may
+    also be one list of ranks per replica of the stage pipeline (`runtime.py --replicas`, no reference equivalent): the
+    data rank, outside every replica, then feeds all of them (`replica_neighbours`)."""
+    if stage_ranks and isinstance(stage_ranks[0], (list, tuple)):
+        if rank == data_rank:
+            assert handle_results_cb is not None
+            if stage is not None:
+                raise ValueError("Data rank must be outside every replica of the stage pipeline")
+            return p2p.DistP2pPipelineStage([ranks[-1] for ranks in stage_ranks], [ranks[0] for ranks in stage_ranks],
+                                            None, handle_results_cb)
+        _, own_stage, rank_src, rank_dst = replica_neighbours(stage_ranks, data_rank, rank)
+        if stage != own_stage:
+            raise ValueError(f"rank {rank} is stage {own_stage} of its replica, not stage {stage}")
+        return p2p.DistP2pPipelineStage(rank_src, rank_dst, module if stage is not None else None, None)
     n_stages = len(stage_ranks)
     if rank == data_rank:
         assert handle_results_cb is not None

@@ -30,7 +30,7 @@ import socket
 import struct
 import threading
 import time
-from typing import Any, Callable, List, Optional, Tuple
+from typing import Any, Callable, List, Optional, Sequence, Tuple, Union
 import ctypes
 import torch
 import torch.distributed as dist
@@ -762,14 +762,25 @@ class DistP2pPipelineStage:
     the last stage's output on the data rank. Thread and queue topology follow the reference's `_create_stage`.
     """
 
-    def __init__(self, rank_src: Optional[int], rank_dst: Optional[int], work_cb: Optional[Callable],
-                 results_cb: Optional[Callable[[Any], None]]):
+    def __init__(self, rank_src: Union[None, int, Sequence[int]], rank_dst: Union[None, int, Sequence[int]],
+                 work_cb: Optional[Callable], results_cb: Optional[Callable[[Any], None]]):
         self._initialized = False
         self._queues = {}
         self._threads = {}
         self._args = (rank_src, rank_dst, work_cb, results_cb)
         self._native = None            # _native.NativeStage once init() has chosen the native pipeline
         self._native_world = False     # every rank agreed on it (then shutdown ends with a drain barrier everywhere)
+        # A data rank outside R replicas of the stage pipeline (no reference equivalent): `rank_src` / `rank_dst` list
+        # each replica's last / first stage. Only the native pipeline serves it (`_native.NativeReplicaFeeder`).
+        self._replicas: Optional[List[Tuple[int, int]]] = None
+        self._replica_timing_hooks: List[Tuple[Callable[..., None], tuple]] = []
+        if isinstance(rank_src, (list, tuple)) or isinstance(rank_dst, (list, tuple)):
+            if work_cb is not None or results_cb is None or not isinstance(rank_src, (list, tuple)) or \
+                    not isinstance(rank_dst, (list, tuple)) or len(rank_src) != len(rank_dst) or not rank_src:
+                raise ValueError("replicas: only a data rank outside the stage pipeline (no worker, a results callback) "
+                                 "takes lists of ranks, one source and one destination per replica")
+            self._replicas = [(int(src), int(dst)) for src, dst in zip(rank_src, rank_dst)]
+            return
         self._create_stage(rank_src, rank_dst, work_cb, results_cb)
 
     # ------------------------------------------------------------------ native pipeline selection
@@ -786,45 +797,60 @@ class DistP2pPipelineStage:
         data rank outside the stage pipeline (no worker, both ranks set), which feeds the first stage through a relay,
         or, without a CUDA device, through a ring in shared memory. A rank without a CUDA device is capable only in
         that role, or idle."""
+        return self._native_refusal() is None
+
+    def _native_refusal(self) -> Optional[str]:
+        """Why THIS rank's role cannot run on the native pipeline (`_native_capable`), or None if it can."""
         rank_src, rank_dst, work_cb, results_cb = self._args
         if os.environ.get('PIPEEDGE_NATIVE', '1') == '0':
-            return False
+            return "PIPEEDGE_NATIVE=0"
         if rank_src is None and rank_dst is None and work_cb is None and results_cb is None:
-            return True    # idle rank: neutral
+            return None    # idle rank: neutral
         if not torch.cuda.is_available() and not self._host_feeder():
-            return False
+            return "no CUDA device"
         try:
             from ._native import shard_is_native   # pylint: disable=import-outside-toplevel
         except ImportError:
-            return False
+            return "the native library cannot be loaded"
         feeder = work_cb is None and results_cb is not None and rank_src is not None and rank_dst is not None
         if not feeder and (work_cb is None or not shard_is_native(work_cb)):
-            return False
+            return "a shard, or a shard hook, that the native pipeline does not support"
         if any(thr._pre_hooks or thr._post_hooks   # pylint: disable=protected-access
                for thr in self._threads.values() if isinstance(thr, AbstractTensorExchangeThread)):
-            return False   # user hooks run on the Python exchange threads (send-timing hooks do not: device timestamps)
+            # user hooks run on the Python exchange threads (send-timing hooks do not: device timestamps)
+            return "exchange hooks"
         if (rank_src is None) != (rank_dst is None):
-            return False
+            return "a stage with only one hop"
         if results_cb is not None and not feeder and not work_cb.shard_config.is_first:
-            return False
-        return True
+            return "a data rank on a stage other than the first"
+        return None
 
     def _choose_native(self) -> bool:
         capable = self._native_capable()
         if dist.is_initialized() and dist.get_world_size() > 1:
-            # Every rank votes, with or without a CUDA device: [capable, -(host feeder), -(has a CUDA device)], MIN.
-            # A data rank without a GPU outside the stage pipeline needs the native pipeline; so does the rest of the
-            # world when any rank has a GPU (a world without one runs the Python threads over Gloo, as before).
+            # Every rank votes, with or without a CUDA device: [capable, -(needs the native pipeline), -(has a CUDA
+            # device)], MIN. A data rank without a GPU outside the stage pipeline needs the native pipeline (-1); so does
+            # the rest of the world when any rank has a GPU (a world without one runs the Python threads over Gloo, as
+            # before). A data rank that feeds replicas needs it in any world (-2): the Python threads run one pipeline.
             host_feeder = self._host_feeder()
-            vote = torch.tensor([1 if capable else 0, -1 if host_feeder else 0, -1 if torch.cuda.is_available() else 0],
-                                dtype=torch.int)
+            need = -2 if self._replicas is not None else -1 if host_feeder else 0
+            vote = torch.tensor([1 if capable else 0, need, -1 if torch.cuda.is_available() else 0], dtype=torch.int)
             dist.all_reduce(vote, op=dist.ReduceOp.MIN)    # control plane (Gloo); every rank builds a stage object
             native = bool(vote[0] == 1)
+            if not native and int(vote[1]) <= -2:
+                # every rank sees this vote: each names its own reason, and every rank raises the same error
+                reasons = [None] * dist.get_world_size()
+                dist.all_gather_object(reasons, self._native_refusal())
+                named = '; '.join(f"rank {r}: {why}" for r, why in enumerate(reasons) if why)
+                raise RuntimeError(f"the data rank feeds pipeline replicas, which only the native pipeline runs, and not "
+                                   f"every rank can run it ({named})")
             if not native and int(vote[1]) < 0 and int(vote[2]) < 0:
                 raise RuntimeError("the data rank has no CUDA device: only the native pipeline can serve it, and not "
                                    "every rank can run it (PIPEEDGE_NATIVE=0, exchange hooks, or a shard it does not "
                                    "support); give the data rank a GPU or run every rank natively")
             return native
+        if self._replicas is not None:
+            raise RuntimeError("a data rank that feeds pipeline replicas needs the replicas' ranks in its process group")
         return capable and self._args[0] is None and self._args[1] is None
 
     def _create_stage(self, rank_src, rank_dst, work_cb, results_cb):
@@ -856,7 +882,10 @@ class DistP2pPipelineStage:
         if self._choose_native():
             self._native_world = True
             rank_src, rank_dst, work_cb, results_cb = self._args
-            if work_cb is not None:
+            if self._replicas is not None:   # the data rank outside R replicas of the stage pipeline
+                from ._native import NativeReplicaFeeder   # pylint: disable=import-outside-toplevel
+                self._native = NativeReplicaFeeder(self._replicas, results_cb, host=not torch.cuda.is_available())
+            elif work_cb is not None:
                 from ._native import NativeStage   # pylint: disable=import-outside-toplevel
                 self._native = NativeStage(rank_src, rank_dst, work_cb, results_cb)
             elif results_cb is not None and self._host_feeder():   # ... outside the stage pipeline, without a GPU
@@ -867,7 +896,8 @@ class DistP2pPipelineStage:
                 self._native = NativeFeeder(rank_src, rank_dst, results_cb)
             if self._native is not None:
                 send = self._threads.get('send')
-                for hook, args in (send._timing_hooks if send is not None else ()):   # pylint: disable=protected-access
+                hooks = send._timing_hooks if send is not None else self._replica_timing_hooks   # pylint: disable=protected-access
+                for hook, args in hooks:
                     self._native.add_send_timing_hook(hook, args)   # registered before init(): stamps from the start
                 self._native.init(DistP2pContext.connect_to, DistP2pContext.accept_from)
             return
@@ -944,11 +974,16 @@ class DistP2pPipelineStage:
             return
         if self._native_world:
             return   # idle rank: it sends nothing
+        if self._replicas is not None:
+            self._replica_timing_hooks.append((hook, args))   # handed to every replica's feeder at init()
+            return
         thr = self._threads.get('send')
         if thr is not None:
             thr.register_timing_hook(hook, args)
 
     def _no_hooks_on_native(self) -> None:
+        if self._replicas is not None:
+            raise RuntimeError("exchange hooks run on the Python exchange threads, which do not feed pipeline replicas")
         if self._native_world:
             raise RuntimeError("the native pipeline is running: register exchange hooks BEFORE init() (they select the "
                                "Python exchange threads) or set PIPEEDGE_NATIVE=0")
@@ -956,7 +991,8 @@ class DistP2pPipelineStage:
     @property
     def native(self):
         """The `_native.NativeStage` driving this rank (a `_native.NativeFeeder` on a data rank outside the stage
-        pipeline, a `_native.NativeHostFeeder` on one without a CUDA device), or None (Python threads / idle rank)."""
+        pipeline, a `_native.NativeHostFeeder` on one without a CUDA device, a `_native.NativeReplicaFeeder` on one that
+        feeds replicas), or None (Python threads / idle rank)."""
         return self._native
 
     def prepare(self, ubatch: int, dim1: int = 0) -> None:

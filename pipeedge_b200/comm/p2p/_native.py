@@ -14,7 +14,9 @@ per-micro-batch host work runs in C with the GIL released:
 * such a data rank without a CUDA device (`NativeHostFeeder`) never touches CUDA: its hops are rings in shared memory
   (`pe_hostring_*`). The last stage's send kernel stores results into one (its `pe_link_open` learns from the
   handshake that the peer is such a ring); the first stage feeds inputs out of the other into a host-fed ring, as a
-  data rank that owns it does (`NativeStage._shm_loop`).
+  data rank that owns it does (`NativeStage._shm_loop`);
+* a data rank outside R replicas of the stage pipeline (`NativeReplicaFeeder`) holds one of those feeders per replica,
+  feeds them round-robin and hands the results on in enqueue order (`InOrderResults`). The stages are unchanged.
 
 Activations cross hops as peer-memory stores synchronised by device-polled flags (`csrc/link.cu`); QuantPipe
 quantisation (`-q`, the shard's `quant_bit` buffer) is fused into the send kernel and undone by the receive kernel, so
@@ -680,8 +682,15 @@ class NativeStage:
         stage thread, then - after ALL ranks have drained (barrier) - unmap the peers' memory and free this rank's."""
         if self._closed:
             return
-        self._closed = True
         failure = self.exception
+        self.drain(timeout)
+        if dist.is_initialized() and dist.get_world_size() > 1 and failure is None and self.exception is None:
+            drain_barrier()   # no rank frees its ring while a neighbour's kernel may still store into it
+        self.release()
+
+    def drain(self, timeout: float = 120.0) -> None:
+        """The first half of `shutdown`: close the input (data rank) and wait until this rank's threads have finished."""
+        self._closed = True
         if self._is_data and self._pipe:
             LIB.pe_pipe_close_input(self._pipe)
         for thr in self._threads:
@@ -691,8 +700,9 @@ class NativeStage:
         if self._drain_thread is not None:
             self._drain_stop.set()      # every graph has completed: the drain thread's last pass reads every record
             self._drain_thread.join(timeout)
-        if dist.is_initialized() and dist.get_world_size() > 1 and failure is None and self.exception is None:
-            drain_barrier()   # no rank frees its ring while a neighbour's kernel may still store into it
+
+    def release(self) -> None:
+        """The second half of `shutdown`, once every rank has drained: free the pipe, links and sockets."""
         if self._pipe:
             LIB.pe_pipe_destroy(self._pipe)
             self._pipe = ctypes.c_void_p()
@@ -722,22 +732,33 @@ class NativeFeeder(NativeStage):
     def init(self, connect_to: Callable, accept_from: Callable) -> None:
         """Open the hop to the first stage (reading its input geometry first) and the hop from the last one, in
         ascending order of the sender's rank like every stage, then the host-fed ring; build the pipe."""
+        for _, _, kind in sorted(self.hops()):
+            self.open_hop(kind, connect_to, accept_from)
+        self.start()
+
+    def hops(self) -> List[Tuple[int, int, str]]:
+        """(sender rank, receiver rank, 'send' | 'recv') of this feeder's two hops."""
         rank = dist.get_rank() if dist.is_initialized() else 0
-        peer_in = peer_out = None
-        for _, kind in sorted([(rank, 'send'), (self._rank_src, 'recv')]):
-            if kind == 'send':
-                sock = connect_to(self._rank_dst)
-                self._socks.append(sock)
-                self._geometry = recv_input_geometry(sock)
-                peer_out = self._open_link(sock, True, self._geometry[0])
-            else:
-                sock = accept_from(self._rank_src)
-                self._socks.append(sock)
-                peer_in = self._open_link(sock, False, 0)
+        return [(rank, self._rank_dst, 'send'), (self._rank_src, rank, 'recv')]
+
+    def open_hop(self, kind: str, connect_to: Callable, accept_from: Callable) -> None:
+        """Open one hop of `hops()` (blocks until the peer joins)."""
+        if kind == 'send':
+            sock = connect_to(self._rank_dst)
+            self._socks.append(sock)
+            self._geometry = recv_input_geometry(sock)
+            self._link_out = self._open_link(sock, True, self._geometry[0])
+        else:
+            sock = accept_from(self._rank_src)
+            self._socks.append(sock)
+            self._link_res = self._open_link(sock, False, 0)
+
+    def start(self) -> None:
+        """Once both hops are open: the host-fed ring, the pipe and the results thread."""
         handle = ctypes.c_void_p()
         check(LIB.pe_link_open_host(self._geometry[0], link_slots(), ctypes.byref(handle)))
         self._links.append(handle)
-        self._link_in, self._link_out, self._link_res = handle, peer_out, peer_in
+        self._link_in = handle
         check(LIB.pe_pipe_create(self._link_in, self._link_out, self._link_res, ctypes.byref(self._pipe)))
         self._stream = torch.cuda.ExternalStream(LIB.pe_pipe_stream(self._pipe), device=self._device)
         self._copy_stream = torch.cuda.ExternalStream(LIB.pe_pipe_copy_stream(self._pipe), device=self._device)
@@ -821,22 +842,35 @@ class NativeHostFeeder:
     def init(self, connect_to: Callable, accept_from: Callable) -> None:
         """Open the hop to the first stage (reading its input geometry first) and the hop from the last one, in
         ascending order of the sender's rank like every stage; start the results thread."""
+        for _, _, kind in sorted(self.hops()):
+            self.open_hop(kind, connect_to, accept_from)
+        self.start()
+
+    def hops(self) -> List[Tuple[int, int, str]]:
+        """(sender rank, receiver rank, 'send' | 'recv') of this feeder's two hops."""
         rank = dist.get_rank() if dist.is_initialized() else 0
-        for _, kind in sorted([(rank, 'send'), (self._rank_src, 'recv')]):
-            handle = ctypes.c_void_p()
-            if kind == 'send':
-                sock = connect_to(self._rank_dst)
-                self._socks.append(sock)
-                self._geometry = recv_input_geometry(sock)
-                check(LIB.pe_hostring_create(sock.fileno(), shm_name(rank, self._rank_dst).encode(), 1,
-                                             self._geometry[0], link_slots(), ctypes.byref(handle)))
-                self._ring_in = handle
-            else:
-                sock = accept_from(self._rank_src)
-                self._socks.append(sock)
-                check(LIB.pe_hostring_create(sock.fileno(), shm_name(self._rank_src, rank).encode(), 0, 0, 0,
-                                             ctypes.byref(handle)))
-                self._ring_res = handle
+        return [(rank, self._rank_dst, 'send'), (self._rank_src, rank, 'recv')]
+
+    def open_hop(self, kind: str, connect_to: Callable, accept_from: Callable) -> None:
+        """Open one hop of `hops()`: create its ring and hand it to the peer (blocks until the peer joins)."""
+        rank = dist.get_rank() if dist.is_initialized() else 0
+        handle = ctypes.c_void_p()
+        if kind == 'send':
+            sock = connect_to(self._rank_dst)
+            self._socks.append(sock)
+            self._geometry = recv_input_geometry(sock)
+            check(LIB.pe_hostring_create(sock.fileno(), shm_name(rank, self._rank_dst).encode(), 1,
+                                         self._geometry[0], link_slots(), ctypes.byref(handle)))
+            self._ring_in = handle
+        else:
+            sock = accept_from(self._rank_src)
+            self._socks.append(sock)
+            check(LIB.pe_hostring_create(sock.fileno(), shm_name(self._rank_src, rank).encode(), 0, 0, 0,
+                                         ctypes.byref(handle)))
+            self._ring_res = handle
+
+    def start(self) -> None:
+        """Once both rings exist: the results thread."""
         self._thread = threading.Thread(target=self._guard, daemon=True, name='pe-host-results')
         self._thread.start()
 
@@ -906,14 +940,22 @@ class NativeHostFeeder:
         after ALL ranks have drained (barrier) - unmap the rings."""
         if self._closed:
             return
-        self._closed = True
         failure = self.exception
+        self.drain(timeout)
+        if dist.is_initialized() and dist.get_world_size() > 1 and failure is None and self.exception is None:
+            drain_barrier()   # no rank unmaps a ring while a neighbour may still use it
+        self.release()
+
+    def drain(self, timeout: float = 120.0) -> None:
+        """The first half of `shutdown`: close the input and wait for the results thread."""
+        self._closed = True
         if self._ring_in:
             LIB.pe_hostring_close_input(self._ring_in)
         if self._thread is not None:
             self._thread.join(timeout)
-        if dist.is_initialized() and dist.get_world_size() > 1 and failure is None and self.exception is None:
-            drain_barrier()   # no rank unmaps a ring while a neighbour may still use it
+
+    def release(self) -> None:
+        """The second half of `shutdown`, once every rank has drained: unmap the rings, close the sockets."""
         for handle in (self._ring_in, self._ring_res):
             if handle:
                 LIB.pe_hostring_close(handle)
@@ -924,3 +966,126 @@ class NativeHostFeeder:
             except OSError:
                 pass
         self._socks.clear()
+
+
+class InOrderResults:
+    """The fan-in of R pipeline replicas fed round-robin: replica k's j-th result is micro-batch j * R + k, and every
+    result reaches `results_cb` in enqueue order, whichever replica finishes first. Each replica's results thread hands
+    its results to `sink(k)`; the result that completes the next micro-batch in order is delivered at once, with the
+    held ones that follow it. Deliveries run under one lock, one at a time. A held result never blocks its replica, and
+    at most what the rings hold is held: the round-robin feed stops at a full replica."""
+
+    def __init__(self, replicas: int, results_cb: Callable):
+        self._replicas = replicas
+        self._results_cb = results_cb
+        self._lock = threading.Lock()
+        self._counts = [0] * replicas     # results received per replica
+        self._held = {}                   # micro-batch index -> result that arrived ahead of its turn
+        self.delivered = 0
+
+    def sink(self, replica: int) -> Callable:
+        """The results callback of replica `replica`."""
+        return lambda result: self._put(replica, result)
+
+    def _put(self, replica: int, result) -> None:
+        with self._lock:
+            self._held[self._counts[replica] * self._replicas + replica] = result
+            self._counts[replica] += 1
+            while self.delivered in self._held:
+                out = self._held.pop(self.delivered)
+                self.delivered += 1
+                self._results_cb(out)
+
+    @property
+    def held(self) -> List[int]:
+        """Micro-batches that arrived but wait for an earlier one (empty once every result has come back)."""
+        with self._lock:
+            return sorted(self._held)
+
+
+class NativeReplicaFeeder:
+    """A data rank outside the stage pipeline that feeds R replicas of it (`runtime.py --replicas R`): one feeder per
+    replica - `NativeFeeder` with a CUDA device, `NativeHostFeeder` without - each owning that replica's two hops.
+    `enqueue` sends micro-batch i to replica i mod R and blocks while that replica's input ring is full (also when
+    another replica has room: the order stays deterministic); `results_cb` receives the results in enqueue order
+    (`InOrderResults`). `pairs`: (rank_src, rank_dst) of each replica, i.e. (its last stage, its first stage).
+    `factory(rank_src, rank_dst, results_cb)` builds one feeder (injectable for tests)."""
+
+    def __init__(self, pairs: List[Tuple[int, int]], results_cb: Callable, host: bool,
+                 factory: Optional[Callable] = None):
+        if not pairs:
+            raise ValueError("native pipeline: a replica feeder needs at least one replica")
+        factory = factory or (NativeHostFeeder if host else NativeFeeder)
+        self._order = InOrderResults(len(pairs), results_cb)
+        self.feeders = [factory(src, dst, self._order.sink(k)) for k, (src, dst) in enumerate(pairs)]
+        self._next = 0              # micro-batches enqueued
+        self._closed = False
+        self._geometry = None
+
+    @property
+    def replicas(self) -> int:
+        """R."""
+        return len(self.feeders)
+
+    def init(self, connect_to: Callable, accept_from: Callable) -> None:
+        """Open every replica's hops in ascending order of (sender, receiver) rank - one global order over all of this
+        rank's hops, as each stage opens its own, so that no two ranks wait for each other - then start the feeders.
+        Refuses replicas whose first stages announce different input geometries."""
+        hops = sorted((sender, receiver, kind, k) for k, feeder in enumerate(self.feeders)
+                      for sender, receiver, kind in feeder.hops())
+        for _, _, kind, k in hops:
+            self.feeders[k].open_hop(kind, connect_to, accept_from)
+        for feeder in self.feeders:
+            feeder.start()
+        geometries = [feeder.input_geometry for feeder in self.feeders]
+        if any(g != geometries[0] for g in geometries):
+            raise ValueError(f"native pipeline: the replicas' first stages take different inputs: {geometries}")
+        self._geometry = geometries[0]
+
+    @property
+    def input_geometry(self) -> Optional[Tuple[int, torch.dtype, int]]:
+        """(largest input micro-batch in bytes, dtype, tensor rank) every replica's first stage announced."""
+        return self._geometry
+
+    def add_send_timing_hook(self, hook: Callable[..., None], args: tuple) -> None:
+        """`hook(mbits, seconds, *args)` once per micro-batch, from whichever replica's feeder sent it."""
+        for feeder in self.feeders:
+            feeder.add_send_timing_hook(hook, args)
+
+    def prepare(self, ubatch: int, dim1: int = 0) -> None:
+        """No-op, as on each feeder."""
+
+    def enqueue(self, tensor: torch.Tensor) -> None:
+        """Insert one micro-batch into the next replica in turn; blocks while that replica's input ring is full."""
+        self.check()
+        self.feeders[self._next % len(self.feeders)].enqueue(tensor)
+        self._next += 1
+
+    @property
+    def delivered(self) -> int:
+        """Results handed to `results_cb` so far."""
+        return self._order.delivered
+
+    def check(self) -> None:
+        """Re-raise what killed any replica's feeder thread."""
+        for feeder in self.feeders:
+            feeder.check()
+
+    def shutdown(self, timeout: float = 120.0) -> None:
+        """Close every replica's input and wait for its results; then - after ALL ranks have drained (one barrier, as
+        every other rank reaches once) - release every feeder."""
+        if self._closed:
+            return
+        self._closed = True
+        failure = any(feeder.exception is not None for feeder in self.feeders)
+        for feeder in self.feeders:
+            feeder.drain(timeout)
+        failure = failure or any(feeder.exception is not None for feeder in self.feeders)
+        if dist.is_initialized() and dist.get_world_size() > 1 and not failure:
+            drain_barrier()
+        for feeder in self.feeders:
+            feeder.release()
+        held = self._order.held
+        if held:
+            logger.error("native pipeline: %d results were never delivered: micro-batch %d did not come back",
+                         len(held), self._order.delivered)

@@ -13,6 +13,8 @@ Scheduler-generated partitions are ingested in the scheduler's own YAML format (
 the reference's `sched-pipeline` binary when it is on PATH with `-sm/-sdt/-sd`). What is NOT carried over (out of scope,
 SURVEY.md section 2): the RPC backend (`-c rpc`), the `sched-pipeline` planner itself, energy monitoring, and the dataset loaders that need the network; inputs are the reference's synthetic fallback (`runtime.py:386-400`)
 generated locally, weights come from `-M` (an npz in the reference layout) or are synthesised.
+One extension the reference lacks: `--replicas R` runs R replicas of the `-pt` pipeline on R*S ranks, fed round-robin by
+a data rank outside all of them, with results in input order (`replica_schedule`, `_native.NativeReplicaFeeder`).
 """
 import argparse
 import logging
@@ -486,6 +488,52 @@ def get_pipeline_sched(world_size: int, partition: Optional[List[Tuple[int, int]
     return stage_layers, stage_quant, stage_ranks
 
 
+def replica_schedule(world_size: int, replicas: int, partition: Optional[List[Tuple[int, int]]],
+                     quant: Optional[List[int]], rank_order: Optional[List[int]], data_rank: int, model_name: str,
+                     automated: bool = False) -> Tuple[List[Tuple[int, int]], List[int], List[List[int]]]:
+    """The schedule of `replicas` (R) replicas of one stage pipeline, fed by the data rank outside all of them (this
+    build's extension, `--replicas`): `stage_layers`, `stage_quant` and `replica_ranks`, where replica k's stage s runs
+    on `replica_ranks[k][s]`. `partition` / `quant` describe one pipeline of S stages (without `partition`, one stage
+    of every layer) that every replica runs; `rank_order` lists R * S ranks replica-major, by default every rank but the
+    data rank in ascending order (the rest stay idle). `automated`: -H / --sched-file / -sm were given. Raises
+    ValueError for a schedule it cannot run."""
+    if replicas < 1:
+        raise ValueError(f"--replicas must be at least 1, got {replicas}")
+    if automated:
+        raise ValueError("--replicas > 1 takes a partition (-pt), not automated scheduling (-H, --sched-file, -sm): "
+                         "the scheduler plans a single pipeline")
+    if partition:
+        stage_layers = list(partition)
+    elif quant:
+        raise ValueError("Must specify partition with quantization")
+    else:
+        stage_layers = [(1, model_cfg.get_model_layers(model_name))]
+    n_stages = len(stage_layers)
+    stage_quant = list(quant) if quant else [0] * n_stages
+    if len(stage_quant) != n_stages:
+        raise ValueError(f"-q lists {len(stage_quant)} bit-widths for a pipeline of {n_stages} stages")
+    if not 0 <= data_rank < world_size:
+        raise ValueError(f"data rank {data_rank} is not a rank of a world of {world_size}")
+    need = replicas * n_stages
+    if world_size < need + 1:
+        raise ValueError(f"{replicas} replicas of {n_stages} stages need {need} ranks plus the data rank; the world "
+                         f"has {world_size}")
+    if rank_order:
+        if len(rank_order) != need:
+            raise ValueError(f"-r lists {len(rank_order)} ranks; {replicas} replicas of {n_stages} stages take {need}")
+    else:
+        rank_order = [r for r in range(world_size) if r != data_rank][:need]
+    if len(set(rank_order)) != len(rank_order):
+        raise ValueError(f"-r lists a rank twice: {rank_order}")
+    outside = [r for r in rank_order if not 0 <= r < world_size]
+    if outside:
+        raise ValueError(f"-r lists ranks outside the world of {world_size}: {outside}")
+    if data_rank in rank_order:
+        raise ValueError(f"data rank {data_rank} is inside a replica; with --replicas it must be outside every one")
+    replica_ranks = [list(rank_order[k * n_stages:(k + 1) * n_stages]) for k in range(replicas)]
+    return stage_layers, stage_quant, replica_ranks
+
+
 def load_dataset(model_name: str, batch_size: int, ubatch_size: int) -> Dataset:
     """Synthetic inputs in place of the reference's downloaded image / `bert_input.npz` (`runtime.py:386-400`)."""
     spec = MODEL_SPECS[model_name]
@@ -522,25 +570,42 @@ def handle_cmd(cmd: int, tensors: Tuple[torch.Tensor, ...]) -> None:
 def run_pipeline_p2p(world_size: int, rank: int, model_name: str, model_file: Optional[str], batch_size: int,
                      ubatch_size: int, partition: Optional[List[Tuple[int, int]]], quant: Optional[List[int]],
                      rank_order: Optional[List[int]], data_rank: int, hosts: Optional[List[str]] = None,
-                     sched_args: Optional[dict] = None) -> float:
-    """Run the pipeline using P2P communication (`runtime.py:418-511`); returns throughput on the data rank."""
+                     sched_args: Optional[dict] = None, replicas: int = 1) -> float:
+    """Run the pipeline using P2P communication (`runtime.py:418-511`); returns throughput on the data rank.
+    `replicas` > 1: that many replicas of the stage pipeline, fed by the data rank outside them (`replica_schedule`)."""
     throughput = 0.0
     monitoring.init(MONITORING_KEY_SEND, get_window_size(), work_type='Mbits')
     if os.getenv(ENV_MONITORING, '0') == '1':
         enable_monitoring()
     with DistP2pContext(('gloo',), {'world_size': world_size, 'rank': rank}, handle_cmd) as dist_ctx:
         if rank == 0:
-            stage_layers, stage_quant, stage_ranks = get_pipeline_sched(world_size, partition, quant, rank_order,
-                                                                        model_name, hosts=hosts,
-                                                                        microbatch_size=ubatch_size, **(sched_args or {}))
+            if replicas > 1:
+                stage_layers, stage_quant, stage_ranks = replica_schedule(
+                    world_size, replicas, partition, quant, rank_order, data_rank, model_name,
+                    automated=bool(hosts or any((sched_args or {}).values())))
+                logger.info("Scheduling: stage-to-layer mapping: %s", stage_layers)
+                logger.info("Scheduling: stage output quantization: %s", stage_quant)
+                logger.info("Scheduling: replica stage-to-rank mapping: %s", stage_ranks)
+            else:
+                stage_layers, stage_quant, stage_ranks = get_pipeline_sched(world_size, partition, quant, rank_order,
+                                                                            model_name, hosts=hosts,
+                                                                            microbatch_size=ubatch_size,
+                                                                            **(sched_args or {}))
+            # with replicas, stage_ranks travels as an R x S tensor: receivers get a list per replica
             dist_ctx.cmd_broadcast(CMD_SCHED, (torch.tensor(stage_layers), torch.tensor(stage_quant),
                                                torch.tensor(stage_ranks), torch.tensor(data_rank)))
         else:
             stage_layers, stage_quant, stage_ranks, data_rank = sched_q.get()
-        try:
-            stage = stage_ranks.index(rank)
-        except ValueError:
-            stage = None
+        replica = None
+        if stage_ranks and isinstance(stage_ranks[0], list):
+            replica, stage, _, _ = model_cfg.replica_neighbours(stage_ranks, data_rank, rank)
+            n_stages = len(stage_ranks[0])
+        else:
+            try:
+                stage = stage_ranks.index(rank)
+            except ValueError:
+                stage = None
+            n_stages = len(stage_ranks)
         check_host_only_role(stage)
         if stage is None:
             model = None
@@ -561,7 +626,7 @@ def run_pipeline_p2p(world_size: int, rank: int, model_name: str, model_file: Op
             model.register_buffer('rate_constraint', torch.tensor(send_constraint), persistent=False)
             model.register_forward_hook(devices.forward_hook_to_cpu)
             model.register_forward_hook(forward_hook_monitor)
-            if stage != len(stage_ranks) - 1:
+            if stage != n_stages - 1:
                 quant_impl = os.getenv(ENV_ADAPTIVE_QUANT)
                 if quant_impl == ADAPTIVE_QUANT_CONTROLLER:
                     model.register_forward_hook(forward_hook_set_quant_controller)
@@ -577,7 +642,15 @@ def run_pipeline_p2p(world_size: int, rank: int, model_name: str, model_file: Op
         with model_cfg.dist_p2p_pipeline_stage_factory(stage_ranks, data_rank, rank, stage, model,
                                                        handle_results) as stage_ctx:
             if model is not None:
-                logger.info("Pipeline stage: %s", 'native' if stage_ctx.native is not None else 'Python threads')
+                path = 'native' if stage_ctx.native is not None else 'Python threads'
+                if replica is None:
+                    logger.info("Pipeline stage: %s", path)
+                else:
+                    logger.info("Pipeline stage: %s (replica %d, stage %d)", path, replica, stage)
+            elif rank == data_rank and isinstance(stage_ranks[0], list):
+                # outside R replicas of the stage pipeline: it feeds every first stage and collects every result
+                logger.info("Data rank: native (%sreplicas %d)", '' if torch.cuda.is_available() else 'host, ',
+                            len(stage_ranks))
             elif rank == data_rank:   # outside the stage pipeline: it feeds the first stage and collects results
                 kind = 'Python threads' if stage_ctx.native is None else \
                     'native (host)' if not torch.cuda.is_available() else 'native'
@@ -661,7 +734,14 @@ def main() -> None:
     usched.add_argument("-q", "--quant", type=str,
                         help="comma-delimited list of quantization bits to use after each stage")
     usched.add_argument("-r", "--rank-order", type=str, default=None,
-                        help="comma-delimited list of ranks in desired stage order; default: natural rank order")
+                        help="comma-delimited list of ranks in desired stage order; default: natural rank order. With "
+                             "--replicas R: R*S ranks, replica-major (replica k's stage s is the (k*S+s)-th); default: "
+                             "every rank but the data rank, ascending")
+    usched.add_argument("--replicas", type=int, default=1,
+                        help="this build's extension (the reference has no such flag): run R replicas of the stage "
+                             "pipeline that -pt / -q describe, fed round-robin by the data rank (-D), which must be "
+                             "outside every replica; results come back in input order. Needs R*S+1 ranks and the "
+                             "native pipeline; not with automated scheduling")
     parser.add_argument("-H", "--hosts", type=str,
                         help="comma-delimited list of hosts in rank order; required for automated scheduling")
     asched = parser.add_argument_group('Automated scheduling')
@@ -683,6 +763,14 @@ def main() -> None:
         partition = [(parts[i], parts[i + 1]) for i in range(0, len(parts), 2)]
     quant = None if args.quant is None else [int(i) for i in args.quant.split(',')]
     rank_order = None if args.rank_order is None else [int(i) for i in args.rank_order.split(',')]
+    hosts = args.hosts.split(',') if args.hosts else None
+    sched_args = {'sched_file': args.sched_file, 's_models_file': args.sched_models_file,
+                  's_dev_types_file': args.sched_dev_types_file, 's_dev_file': args.sched_dev_file}
+    if args.replicas != 1:
+        # every rank checks its own command line before joining the world: a schedule rank 0 would refuse then stops
+        # every rank, instead of leaving the others waiting for it
+        replica_schedule(args.worldsize, args.replicas, partition, quant, rank_order, args.data_rank, args.model_name,
+                         automated=bool(hosts or any(sched_args.values())))
 
     tik = time.time()
     device = args.device
@@ -690,11 +778,9 @@ def main() -> None:
         device = f"cuda:{args.rank % max(1, torch.cuda.device_count())}"
     init_env(device, args.addr, args.port, args.socket_ifname if args.socket_ifname != 'lo0' else '')
     logger.info("Device: %s", devices.DEVICE)
-    hosts = args.hosts.split(',') if args.hosts else None
     run_pipeline_p2p(args.worldsize, args.rank, args.model_name, args.model_file, args.batch_size,
                      args.ubatch_size, partition, quant, rank_order, args.data_rank, hosts=hosts,
-                     sched_args={'sched_file': args.sched_file, 's_models_file': args.sched_models_file,
-                                 's_dev_types_file': args.sched_dev_types_file, 's_dev_file': args.sched_dev_file})
+                     sched_args=sched_args, replicas=args.replicas)
     logger.info("Total program execution time = %f", time.time() - tik)
 
 
