@@ -201,6 +201,21 @@ int pe_stage_profile(pe_stage* stage, const void* in0, const void* in1, void* ou
                      void* stream, float* ms_out, int* kinds_out, int capacity, int* n_out);
 /* Number of kernels one pe_stage_forward enqueues for `ubatch` items (for bench.py's gpu_launches). */
 int pe_stage_kernel_count(const pe_stage* stage);
+/* Sub-layer timestamps (the profiler's in-context times). While `stamps` is not NULL, every pe_stage_forward, eager or
+ * captured, launches a one-thread kernel after each sub-layer k of the stage (0-based) that writes %globaltimer (ns)
+ * into stamps[row * cols + col0 + k], with row = *row_ctr (device memory, caller-owned like `stamps`). The stamp in
+ * column cols - 1 then advances *row_ctr, so K graph replays fill K rows; rows >= `rows` are counted but not
+ * written. The stamps are plain launches and the PDL kernel after each waits for it. A sub-layer's boundary follows
+ * the last kernel doing its own work: a residual add folded into the next LayerNorm belongs to the next sub-layer,
+ * a projection fused with the next LayerNorm (PE_FUSE_LN=1) to the projection, the stage's entry / exit casts and
+ * final residual add to its first / last sub-layer. Graphs are cached per stamps setting: one captured with other
+ * stamps (or none) is never replayed. `stamps` NULL turns them off; with them off a forward is unchanged. */
+int pe_stage_set_stamps(pe_stage* stage, unsigned long long* stamps, unsigned long long* row_ctr, int rows, int cols,
+                        int col0);
+/* The same stamp on its own: column `col` of row *row_ctr, then *row_ctr += 1 if `bump_row` (e.g. before a first
+ * stage's embeddings and after a last stage's head). */
+int pe_stamp(unsigned long long* stamps, unsigned long long* row_ctr, int rows, int cols, int col, int bump_row,
+             void* stream);
 
 /* ---- Stage-0 edges (SURVEY.md 8a-A13) ------------------------------------------------------------
  * pe_patch_embed replaces HF `ViTEmbeddings` / `DeiTEmbeddings` as used at `vit.py:96,165`, `deit.py:95,161`:

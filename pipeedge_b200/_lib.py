@@ -73,6 +73,8 @@ SYMBOLS = {
                                  POINTER(c_int)]),
     'pe_stage_kernel_count': (c_int, [c_void_p]),
     'pe_stage_deferred': (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_void_p)]),
+    'pe_stage_set_stamps': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int]),
+    'pe_stamp': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     'pe_patch_embed': (c_int, [c_void_p] * 7 + [c_int] * 6 + [c_void_p]),
     'pe_bert_embed': (c_int, [c_void_p] * 7 + [c_float, c_void_p, c_int, c_int, c_int, c_void_p]),
     'pe_hop_available': (c_int, []),

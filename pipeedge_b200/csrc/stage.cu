@@ -43,6 +43,19 @@ struct SubRange {
   int s0, s1; // sub-layers 0..3 inclusive
 };
 
+// Where sub-layer timestamps go (pe_stage_set_stamps / pe_stamp): %globaltimer of boundary `col` of forward *row_ctr
+// at stamps[row * cols + col]; rows past `rows` are counted but not written.
+struct StampTable {
+  unsigned long long* stamps = nullptr;   // nullptr: stamps off
+  unsigned long long* row_ctr = nullptr;
+  int rows = 0, cols = 0, col0 = 0;
+  bool operator<(const StampTable& o) const {
+    return std::tie(stamps, row_ctr, rows, cols, col0) < std::tie(o.stamps, o.row_ctr, o.rows, o.cols, o.col0);
+  }
+  bool operator==(const StampTable& o) const { return !(*this < o) && !(o < *this); }
+};
+int stamp_impl(const StampTable& t, int col, bool bump_row, cudaStream_t stream);
+
 }  // namespace pe
 
 struct pe_stage {
@@ -58,10 +71,13 @@ struct pe_stage {
   const void* defer_a = nullptr;   // PE_STAGE_DEFER_ADD: the stage's output is defer_a + defer_b, left to the consumer
   const void* defer_b = nullptr;
   cudaStream_t capture_stream = nullptr;  // private stream the kernel sequence is captured on
-  typedef std::tuple<int, const void*, const void*, void*, void*> Key;
+  pe::StampTable stamps;                  // sub-layer timestamps of every forward (off unless stamps.stamps is set)
+  // a graph is keyed on the stamps setting too, so turning stamps on or off never replays one captured the other way
+  typedef std::tuple<int, const void*, const void*, void*, void*, pe::StampTable> Key;
   struct Cached {
     cudaGraphExec_t exec = nullptr;
     bool warmed = false;
+    int kernels = 0;   // kernels in the graph
   };
   std::map<Key, Cached> graphs;
 };
@@ -102,9 +118,32 @@ static int lin(const void* a, const void* w, const void* b, const void* resid, v
   return linear_impl(a, w, b, resid, out, m, n, k, epi, 0, 0, 0, 0, /*static_w=*/1, s);
 }
 
-// Enqueue the kernel sequence of one forward on `stream`. Returns the number of kernels in *count.
+// One-thread kernel: %globaltimer into column `col` of the current row; `bump_row` then advances the row. Launched
+// WITHOUT programmatic dependent launch, so it starts only after the kernel before it has completed; the PDL-launched
+// kernel after it waits (griddepcontrol.wait) for the stamp's completion, as pipe.cu's stamps do.
+__global__ void __launch_bounds__(1) stage_stamp_kernel(unsigned long long* stamps, unsigned long long* row_ctr, int rows,
+                                                        int cols, int col, int bump_row) {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  const unsigned long long r = *row_ctr;
+  if (r < static_cast<unsigned long long>(rows)) stamps[r * cols + col] = t;
+  if (bump_row) *row_ctr = r + 1;
+}
+
+int stamp_impl(const StampTable& t, int col, bool bump_row, cudaStream_t stream) {
+  stage_stamp_kernel<<<1, 1, 0, stream>>>(t.stamps, t.row_ctr, t.rows, t.cols, col, bump_row ? 1 : 0);
+  PE_CUDA(cudaGetLastError());
+  count_launches(1);
+  return PE_OK;
+}
+
+// Enqueue the kernel sequence of one forward on `stream`. Returns the number of kernels in *count. With `stamps` on,
+// a stamp follows each sub-layer k of the stage (column col0 + k; the one in the row's last column advances the row).
+// A sub-layer's boundary sits after the last kernel doing its own work: a residual add deferred into the next
+// sub-layer's LayerNorm is charged to that next sub-layer, a projection that also computes the next LayerNorm
+// (PE_FUSE_LN=1) to the projection, and the stage's own entry casts / exit add and casts to its first / last sub-layer.
 static int enqueue(pe_stage* st, const void* in0, const void* in1, void* out0, void* out1, int ubatch,
-                   cudaStream_t stream, int* count, Prof* prof = nullptr, bool defer_add = false) {
+                   cudaStream_t stream, int* count, Prof* prof = nullptr, bool defer_add = false, bool stamps = false) {
   const pe_stage_desc& d = st->d;
   const int H = d.hidden, I = d.inter, S = d.tokens;
   const int M = ubatch * S;
@@ -116,6 +155,12 @@ static int enqueue(pe_stage* st, const void* in0, const void* in1, void* out0, v
   PE_REQUIRE(!in_tuple || in1, "pe_stage_forward: stage starts mid-block and needs the (data, skip) tuple");
   PE_REQUIRE(!out_tuple || out1, "pe_stage_forward: stage ends mid-block and produces a (data, skip) tuple");
   int n_k = 0;
+  int n_sub = 0;   // sub-layers done
+  const StampTable& stamp_to = st->stamps;
+  auto stamp = [&]() {
+    const int col = stamp_to.col0 + n_sub++;
+    return stamps ? stamp_impl(stamp_to, col, col == stamp_to.cols - 1, stream) : PE_OK;
+  };
 
   // every residual-stream write lands in the buffer that finally carries it out of the stage
   float* resid_dest = static_cast<float*>(out_tuple ? out1 : out0);
@@ -213,6 +258,10 @@ static int enqueue(pe_stage* st, const void* in0, const void* in1, void* out0, v
           break;
         }
       }
+      if (has_next) {
+        PE_TRY(stamp());
+        if (stamps) ++n_k;
+      }
     }
   }
   st->defer_a = st->defer_b = nullptr;
@@ -234,6 +283,8 @@ static int enqueue(pe_stage* st, const void* in0, const void* in1, void* out0, v
       PE_CUDA(cudaMemcpyAsync(out1, skip, static_cast<size_t>(M) * H * sizeof(float), cudaMemcpyDeviceToDevice, stream));
     }
   }
+  PE_TRY(stamp());   // the last sub-layer's boundary, after the stage's exit work
+  if (stamps) ++n_k;
   *count = n_k;
   return PE_OK;
 }
@@ -334,24 +385,27 @@ int pe_stage_forward(pe_stage* st, const void* in0, const void* in1, void* out0,
   PE_REQUIRE(ubatch > 0 && ubatch <= st->d.max_ubatch, "pe_stage_forward: ubatch=%d outside [1,%d]", ubatch,
              st->d.max_ubatch);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  const bool stamps = st->stamps.stamps != nullptr;
   if ((use_graph & 1) == 0)
-    return enqueue(st, in0, in1, out0, out1, ubatch, stream, &st->kernels_last, nullptr, (use_graph & PE_STAGE_DEFER_ADD) != 0);
+    return enqueue(st, in0, in1, out0, out1, ubatch, stream, &st->kernels_last, nullptr, (use_graph & PE_STAGE_DEFER_ADD) != 0,
+                   stamps);
 
-  pe_stage::Cached& c = st->graphs[pe_stage::Key(ubatch, in0, in1, out0, out1)];
+  pe_stage::Cached& c = st->graphs[pe_stage::Key(ubatch, in0, in1, out0, out1, st->stamps)];
   if (c.exec != nullptr) {
     PE_CUDA(cudaGraphLaunch(c.exec, stream));
-    count_launches(st->kernels_last);
+    st->kernels_last = c.kernels;
+    count_launches(c.kernels);
     return PE_OK;
   }
   if (!c.warmed) {
     // first use: run eagerly (one-time cudaFuncSetAttribute / driver entry-point lookups happen here)
     c.warmed = true;
-    return enqueue(st, in0, in1, out0, out1, ubatch, stream, &st->kernels_last);
+    return enqueue(st, in0, in1, out0, out1, ubatch, stream, &st->kernels_last, nullptr, false, stamps);
   }
   // second use: capture the same sequence on the stage's private stream (the caller's stream may be the
   // legacy default stream, which cannot be captured), instantiate, then launch into the caller's stream
   if (st->graphs.size() > 64) {  // pointers that never repeat would grow the cache without bound: start over
-    const pe_stage::Key mine(ubatch, in0, in1, out0, out1);
+    const pe_stage::Key mine(ubatch, in0, in1, out0, out1, st->stamps);
     for (auto it = st->graphs.begin(); it != st->graphs.end();) {
       if (it->first == mine) { ++it; continue; }
       if (it->second.exec != nullptr) cudaGraphExecDestroy(it->second.exec);
@@ -362,7 +416,7 @@ int pe_stage_forward(pe_stage* st, const void* in0, const void* in1, void* out0,
   cudaGraph_t graph = nullptr;
   PE_CUDA(cudaStreamBeginCapture(st->capture_stream, cudaStreamCaptureModeThreadLocal));
   int n_k = 0;
-  const int rc = enqueue(st, in0, in1, out0, out1, ubatch, st->capture_stream, &n_k);
+  const int rc = enqueue(st, in0, in1, out0, out1, ubatch, st->capture_stream, &n_k, nullptr, false, stamps);
   const cudaError_t end = cudaStreamEndCapture(st->capture_stream, &graph);
   if (rc != PE_OK) {
     if (graph != nullptr) cudaGraphDestroy(graph);
@@ -372,7 +426,7 @@ int pe_stage_forward(pe_stage* st, const void* in0, const void* in1, void* out0,
   const cudaError_t inst = cudaGraphInstantiate(&c.exec, graph, 0);
   cudaGraphDestroy(graph);
   PE_CUDA(inst);
-  st->kernels_last = n_k;
+  st->kernels_last = c.kernels = n_k;
   PE_CUDA(cudaGraphLaunch(c.exec, stream));
   return PE_OK;  // kernels were already counted by enqueue() during capture
 }
@@ -409,6 +463,40 @@ int pe_stage_profile(pe_stage* st, const void* in0, const void* in1, void* out0,
 }
 
 int pe_stage_kernel_count(const pe_stage* st) { return st == nullptr ? 0 : st->kernels_last; }
+
+int pe_stage_set_stamps(pe_stage* st, unsigned long long* stamps, unsigned long long* row_ctr, int rows, int cols, int col0) {
+  using namespace pe;
+  PE_REQUIRE(st != nullptr, "pe_stage_set_stamps: null stage");
+  if (stamps == nullptr) {
+    st->stamps = StampTable();
+    return PE_OK;
+  }
+  const int n_sub = st->d.layer_end - st->d.layer_start + 1;
+  PE_REQUIRE(row_ctr != nullptr && rows > 0 && col0 >= 0 && col0 + n_sub <= cols,
+             "pe_stage_set_stamps: %d sub-layers from column %d do not fit rows of %d columns (rows=%d, row_ctr=%p)",
+             n_sub, col0, cols, rows, static_cast<void*>(row_ctr));
+  StampTable t;
+  t.stamps = stamps;
+  t.row_ctr = row_ctr;
+  t.rows = rows;
+  t.cols = cols;
+  t.col0 = col0;
+  st->stamps = t;
+  return PE_OK;
+}
+
+int pe_stamp(unsigned long long* stamps, unsigned long long* row_ctr, int rows, int cols, int col, int bump_row,
+             void* stream) {
+  using namespace pe;
+  PE_REQUIRE(stamps != nullptr && row_ctr != nullptr && rows > 0 && col >= 0 && col < cols,
+             "pe_stamp: bad table (rows=%d, cols=%d, col=%d)", rows, cols, col);
+  StampTable t;
+  t.stamps = stamps;
+  t.row_ctr = row_ctr;
+  t.rows = rows;
+  t.cols = cols;
+  return stamp_impl(t, col, bump_row != 0, static_cast<cudaStream_t>(stream));
+}
 
 int pe_stage_deferred(const pe_stage* st, const void** a, const void** b) {
   using namespace pe;

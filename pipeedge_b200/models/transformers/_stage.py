@@ -126,6 +126,7 @@ class EncoderStage:
                 self._tensors.append(t)
                 setattr(blocks[idx], key, t.data_ptr())
         self._blocks = blocks
+        self._stamps = None   # (stamps, row_ctr, col0) of set_stamps
         self._handle = ctypes.c_void_p()
         self._create()
 
@@ -133,6 +134,37 @@ class EncoderStage:
         desc = StageDesc(_lib.PE_FAMILY[self.family], self.hidden, self.heads, self.inter, self.tokens, self.eps,
                          self.layer_start, self.layer_end, self.max_ubatch)
         check(LIB.pe_stage_create(ctypes.byref(desc), self._blocks, len(self.ranges), ctypes.byref(self._handle)))
+        if self._stamps is not None:
+            self.set_stamps(*self._stamps)
+
+    @staticmethod
+    def _check_stamp_table(stamps: torch.Tensor, row_ctr: torch.Tensor) -> None:
+        if not (stamps.is_cuda and stamps.dtype == torch.int64 and stamps.dim() == 2 and stamps.is_contiguous()):
+            raise ValueError("stamps must be a contiguous int64 CUDA tensor [rows, cols]")
+        if not (row_ctr.is_cuda and row_ctr.dtype == torch.int64 and row_ctr.numel() >= 1):
+            raise ValueError("row_ctr must be an int64 CUDA tensor of one element")
+
+    def set_stamps(self, stamps: Optional[torch.Tensor], row_ctr: Optional[torch.Tensor] = None, col0: int = 0) -> None:
+        """Timestamp every later forward after each sub-layer k of the stage: %globaltimer (ns) into
+        `stamps[row_ctr[0], col0 + k]`; the stamp in the last column advances `row_ctr[0]` (pe_stage_set_stamps).
+        `stamps` is an int64 CUDA tensor [rows, cols], `row_ctr` an int64 CUDA tensor holding the next row; the stage
+        keeps references to both. None turns stamps off."""
+        if stamps is None:
+            self._stamps = None
+            check(LIB.pe_stage_set_stamps(self._handle, None, None, 0, 0, 0))
+            return
+        self._check_stamp_table(stamps, row_ctr)
+        check(LIB.pe_stage_set_stamps(self._handle, stamps.data_ptr(), row_ctr.data_ptr(), stamps.shape[0],
+                                      stamps.shape[1], int(col0)))
+        self._stamps = (stamps, row_ctr, int(col0))
+
+    @staticmethod
+    def stamp(stamps: torch.Tensor, row_ctr: torch.Tensor, col: int, bump_row: bool = False) -> None:
+        """One stand-alone stamp on the current stream into `stamps[row_ctr[0], col]`, then advance the row if
+        `bump_row` (pe_stamp): what a shard charges to its first / last sub-layer outside the stage (embeddings, head)."""
+        EncoderStage._check_stamp_table(stamps, row_ctr)
+        check(LIB.pe_stamp(stamps.data_ptr(), row_ctr.data_ptr(), stamps.shape[0], stamps.shape[1], int(col),
+                           1 if bump_row else 0, torch.cuda.current_stream().cuda_stream))
 
     def resize(self, tokens: int, max_ubatch: int) -> None:
         """Re-create the workspace for a different sequence length / micro-batch bound (BERT inputs vary)."""
